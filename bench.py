@@ -2,7 +2,7 @@
 """Headline benchmark: VNet3d(1,2) 96^3, batch 2 per GPU, bf16 storage, forward + loss + backward
 (+ gradient all-reduce for N > 1) in voxels/second (BASELINE.json `metric`, config[1] / config[3]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--no-graph]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--no-graph] [--dump-outputs DIR]
 
 N > 1 is launched by the driver as ``python -m torch.distributed.run --nproc-per-node N bench.py --gpus N``
 (one rank per GPU, NCCL).  Rank 0 prints ONE JSON line.  A "step" = one pass of the hot path
@@ -103,7 +103,9 @@ def oracle_step_fn():
         logits, _ = fwd(sd, x, draw(x.shape[0]))
         loss = oracle.loss_forward(LOSS, logits, y, alpha)
         loss.backward()
-        return float(loss.detach())
+        step.loss = loss.detach()
+        return float(step.loss)
+    step.params = list(sd.values())
     return step
 
 
@@ -114,8 +116,8 @@ def load_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "bf16_tflops_burst": d["bf16_tflops"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "bf16_tflops_burst": 1590.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_burst": 989.0,
+            "source": "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16)"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -228,16 +230,16 @@ class TimedBackend:
     def _describe(name, a):
         if name == "conv":
             kind, dims, x, wpk, bias, y = a[:6]
-            path = {2: "/tcgen05", 3: "/tcgen05-halo", 4: "/tcgen05-halo-ws"}.get(getattr(wpk, "code", 0), "/cuda-core")
+            path = {2: "/wgmma", 3: "/wgmma-halo", 4: "/wgmma-halo-ws"}.get(getattr(wpk, "code", 0), "/cuda-core")
             if x.shape[-1] == 1 and y.dtype == torch.bfloat16:
                 path = "/mma.sync-stem"
             elif (kind in (1, 3) and getattr(wpk, "code", 0) == 2 and max(x.shape[-1], y.shape[-1]) <= 64
                   and y.numel() // y.shape[-1] >= 65536 and x.shape[-1] * y.shape[-1] <= (512 if kind == 3 else 2048)):
-                path = "/mma.sync-pointwise"      # pw_mma.cu takes these shapes ahead of the tcgen05 kernel
+                path = "/mma.sync-pointwise"      # pw_mma.cu takes these shapes ahead of the wgmma kernel
             return f"conv[k{kind}{path}] {x.shape[-1]}->{y.shape[-1]}@{tuple(y.shape[1:4])}"
         if name == "conv_bwdstats":
             kind, dims, x, wpk, y = a[:5]
-            return f"conv+gn_bwd_sums[k{kind}/tcgen05-halo] {x.shape[-1]}->{y.shape[-1]}@{tuple(y.shape[1:4])}"
+            return f"conv+gn_bwd_sums[k{kind}/wgmma-halo] {x.shape[-1]}->{y.shape[-1]}@{tuple(y.shape[1:4])}"
         if name == "wgrad":
             kind, dims, x, dy = a[:4]
             return f"wgrad[k{kind}] {x.shape[-1]}x{dy.shape[-1]}@{tuple(dy.shape[1:4])}"
@@ -297,6 +299,32 @@ def make_batch(rank: int, world: int):
     return x[sl].contiguous(), y[sl].contiguous()
 
 
+DUMP_GRAD_SAMPLE = 4 * 1024 * 1024      # gradient elements kept in the dump (16 MB as float32)
+
+
+def dump_outputs(out_dir, loss, params, graphed=None):
+    """loss, Dice and probs if computed, gradient norms and a fixed (seed 0) sample of the gradient elements"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    outs = {"loss": loss.detach().double().reshape(1)}
+    if graphed is not None and graphed.dice is not None:
+        outs["dice"] = graphed.dice.detach().double().reshape(1)
+    if graphed is not None and graphed.probs is not None:
+        outs["probs"] = graphed.probs.detach().float()
+    grads = [p.grad.detach().float().reshape(-1) if p.grad is not None else torch.zeros(p.numel(), device=p.device)
+             for p in params]
+    outs["grad_norms"] = torch.stack([g.double().norm() for g in grads])
+    flat = torch.cat(grads)
+    if flat.numel() > DUMP_GRAD_SAMPLE:
+        gen = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=gen)[:DUMP_GRAD_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    outs["grad_sample"] = flat
+    for name, t in outs.items():
+        a = t.cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
+
+
 def run_reference(args):
     """The reference's own CPU path for this metric: the oracle restatement (kind 'port') on all host cores."""
     import oracle
@@ -308,7 +336,7 @@ def run_reference(args):
     torch.set_num_threads(cores)
     step = oracle_step_fn()
 
-    steps, warm = max(1, min(args.steps, 5)), max(1, min(args.warmup, 2))
+    steps, warm = args.steps, args.warmup
     for _ in range(warm):
         step()
     ts = []
@@ -316,6 +344,8 @@ def run_reference(args):
         t0 = time.perf_counter()
         step()
         ts.append(time.perf_counter() - t0)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, step.loss, step.params)
     t = statistics.median(ts)
     vox = BATCH_PER_GPU * voxels_per_sample()
     val = vox / t
@@ -393,9 +423,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-variants", action="store_true", help="skip the fwd-only / optimizer / fp32 variants (N=1)")
     ap.add_argument("--workload", default="vnet3d96", choices=sorted(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     _capture_stdout()
     select_workload(args.workload)
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(3, args.warmup)
 
     if args.impl == "reference":
@@ -512,11 +546,13 @@ def main():
         torch.cuda.synchronize()
         return [a.elapsed_time(b) for a, b in evs]
 
+    last = {}
+
     def resident_step():
         if use_graph:
-            graphed()                      # replays on the static (HBM-resident) input buffers
+            last["loss"] = graphed()       # replays on the static (HBM-resident) input buffers
         else:
-            eager_step(x, y)
+            last["loss"] = eager_step(x, y)
 
     host_losses = [torch.empty((), dtype=torch.float32).pin_memory() for _ in range(2)]
     loss_values = []
@@ -559,6 +595,8 @@ def main():
     ms = timed(resident_step, args.steps)
     barrier()
     wall = time.perf_counter() - wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], model.parameters(), graphed)
     clocks = sampler.stop()
     if sum(ms) * 1e-3 > wall * 1.02 + 1e-3:
         raise SystemExit(f"[bench] rank {rank}: inconsistent timing: event sum {sum(ms):.2f} ms > wall {wall * 1e3:.2f} ms")

@@ -1,5 +1,5 @@
 /*
- * b200seg.h -- C ABI of the B200-native (sm_100a) segmentation hot path.
+ * b200seg.h -- C ABI of the H100-native (sm_90a) segmentation hot path.
  *
  * The reference (junqiangchen/PytorchDeepLearing) has NO native code and NO FFI: its "plugin
  * boundary" is the Python nn.Module protocol used by model/modelVNet.py:490-497,546-548,580-593
@@ -35,7 +35,7 @@ extern "C" {
 
 #define B200SEG_F32 0
 #define B200SEG_BF16 1
-#define B200SEG_BF16_TC 2 /* weights only: bf16 packed [tap][N][K] (K-major) for the tcgen05/TMA conv path */
+#define B200SEG_BF16_TC 2 /* weights only: bf16 packed [tap][N][K] (K-major) for the wgmma/TMA conv path */
 #define B200SEG_BF16_HALO 3 /* weights only: bf16 packed [tap][K/8][N][8] (smem image of the halo-staged 3x3x3 path) */
 #define B200SEG_BF16_HALO_WS 4 /* weights only: bf16 packed [N/NT][tap][K/8][NT][8], NT = b200seg_conv_halo_ws_ntile():
                                   per-group tap blocks streamed by the 64/128-channel halo-staged 3x3x3 path */
@@ -123,15 +123,15 @@ int b200seg_conv_bwdstats(int kind, int dims, const b200seg_tensor* x, const voi
                           const b200seg_tensor* y, const b200seg_tensor* addend, const b200seg_tensor* yfwd,
                           const struct b200seg_gn* gn, double* sums, int device, b200seg_stream stream);
 
-/* 1 if b200seg_conv runs (kind, Cin -> Cout) on the tcgen05 + TMA path when given bf16 activations and
+/* 1 if b200seg_conv runs (kind, Cin -> Cout) on the wgmma + TMA path when given bf16 activations and
  * B200SEG_BF16_TC weights ([tap][Cout][Cin] for the forward form, [tap'][Cin][Cout], taps flipped, for the
  * data-gradient form); 0 -> pack [tap][K][N] and use the CUDA-core path. */
 int b200seg_conv_tc_eligible(int kind, int cin, int cout);
-/* 1 if (kind, Cin -> Cout) can run on the halo-staged tcgen05 kernel (3x3x3 / 3x3, 16/32 channels) given
+/* 1 if (kind, Cin -> Cout) can run on the halo-staged wgmma kernel (3x3x3 / 3x3, 16/32 channels) given
  * B200SEG_BF16_HALO weights; meant for the full-resolution layers (each input voxel is staged once in shared
  * memory instead of once per tap). */
 int b200seg_conv_halo_eligible(int kind, int cin, int cout);
-/* columns per weight group (NT) if (kind, Cin -> Cout) can run on the weight-streaming halo-staged tcgen05 kernel
+/* columns per weight group (NT) if (kind, Cin -> Cout) can run on the weight-streaming halo-staged wgmma kernel
  * (3x3x3, 64/128 input channels: the 24^3 / 12^3 pyramid levels) given B200SEG_BF16_HALO_WS weights, else 0. */
 int b200seg_conv_halo_ws_ntile(int kind, int cin, int cout);
 

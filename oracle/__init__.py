@@ -13,7 +13,7 @@ README.md:13 says "pytorch1.10.0"; installed here: torch 2.11.0).
 
 Pinning: the reference ships no tests and no golden vectors (SURVEY.md section 4), so the
 oracle is pinned against OUTPUTS OF THE REFERENCE ITSELF run in the build container:
-``tests/golden/make_golden.py`` imports ``/root/reference`` (with the non-invasive
+``tests/golden/make_golden.py`` imports the reference checkout (``$PYTORCHDEEPLEARING_REFERENCE``) (with the non-invasive
 ``VNet3d`` constructor shim for the ``networks/VNet3d.py:127`` typo), runs it on seeded
 inputs and commits the results as ``tests/golden/*.npz``;  ``tests/test_oracle_golden.py``
 checks this restatement against those fixtures on every CPU run.

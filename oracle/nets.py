@@ -2,7 +2,7 @@
 
 Every function takes a ``state_dict``-style mapping (reference key names, App. A of
 SURVEY.md) and plain tensors; autograd gives the backward pass.  Citations are to
-``/root/reference`` files.
+the reference checkout (``$PYTORCHDEEPLEARING_REFERENCE``) files.
 
 Dropout: ``nn.Dropout3d/2d(p=0.2)`` in train mode multiplies by a per-(sample, channel)
 Bernoulli(0.8)/0.8 scale drawn as ``x.new_empty((N,C,1,1,1)).bernoulli_(0.8).div_(0.8)``

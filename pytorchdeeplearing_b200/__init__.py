@@ -1,4 +1,4 @@
-"""pytorchdeeplearing_b200 -- B200-native (sm_100a) drop-in for the segmentation hot path of
+"""pytorchdeeplearing_b200 -- H100-native (sm_90a) drop-in for the segmentation hot path of
 junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
 ``networks/Unet2d.py`` forward/backward and the Dice / BCE / focal / CE reductions of
 ``model/losses.py`` (SURVEY.md section 8).

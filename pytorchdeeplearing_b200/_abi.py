@@ -154,7 +154,7 @@ def _ref(d):
 
 class PackedWeight:
     """Packed conv operand + its layout code (B200SEG_F32 / BF16 = [tap][K][N]; BF16_TC = [tap][N][K] K-major
-    for the tcgen05 path).  Keeps what is needed to re-pack for the CUDA-core path."""
+    for the wgmma path).  Keeps what is needed to re-pack for the CUDA-core path."""
     __slots__ = ("t", "code", "src", "kind", "which", "dims")
 
     def __init__(self, t, code, src, kind, which, dims):
@@ -169,11 +169,11 @@ class _PackPlan:
 
 
 class CudaBackend:
-    name = "cuda-sm100a"
+    name = "cuda-sm90a"
 
     def __init__(self):
         if not torch.cuda.is_available():
-            raise RuntimeError("pytorchdeeplearing_b200 needs a CUDA device (built for sm_100a); none is available "
+            raise RuntimeError("pytorchdeeplearing_b200 needs a CUDA device (built for sm_90a); none is available "
                                "and there is no CPU fallback")
         self.lib = load_library()
         self._inited = set()
@@ -234,7 +234,7 @@ class CudaBackend:
                 op = {K3: (K3, a, b), K1: (K1, a, b), DOWN: (UP, a, b), UP: (DOWN, b, a)}[kind]
             tc = bool(self.lib.b200seg_conv_tc_eligible(*op))
         if tc:
-            # K-major rows for the tcgen05 path: [tap][N][K]
+            # K-major rows for the wgmma path: [tap][N][K]
             gather_like = (which == "fwd" and kind != UP) or (which == "dgrad" and kind == UP)
             if which == "dgrad" and kind in (K3, K1):      # [T-1-t][ci][co]
                 return (t, b, a), BF16_TC, (t, b, 1, a, 1, t, 0, b * t, 1)
@@ -354,7 +354,7 @@ class CudaBackend:
     def conv(self, kind, dims, x, wpk, bias, y, stats, addend):
         dev, st = self._ds(x)
         if wpk.code in (BF16_TC, BF16_HALO, BF16_HALO_WS) and not (x.dtype == torch.bfloat16 and y.dtype == torch.bfloat16):
-            # tcgen05 path needs bf16 activations on both sides (e.g. a 16-channel fp32 network input)
+            # wgmma path needs bf16 activations on both sides (e.g. a 16-channel fp32 network input)
             wpk = self.pack_weight(wpk.src, wpk.kind, wpk.which, torch.bfloat16, wpk.dims, allow_tc=False)
         dx, dy, da = _desc(x), _desc(y), _desc(addend)
         self._check(self.lib.b200seg_conv(kind, dims, C.byref(dx), wpk.t.data_ptr(), wpk.code, _p(bias), C.byref(dy),
@@ -367,9 +367,8 @@ class CudaBackend:
         if (not self.fused_bwd_stats or wpk.code not in (BF16_HALO, BF16_HALO_WS) or x.dtype != torch.bfloat16
                 or y.dtype != torch.bfloat16):
             return False
-        # measured on B200 (VNet3d 96^3 step): with 32 output channels the fused form beats conv + reduce (42 vs
-        # 33.5 + 19.5 us at 48^3); with 16 it loses (125 vs 60 + 34 us at 96^3: the two-CTA kernel has no registers to
-        # spare and the layer is traffic bound once it also reads the producer's raw output)
+        # with 16 output channels the layer is traffic bound once it also reads the producer's raw output, so the
+        # fused form is used for 32 output channels only (B200SEG_BWDSTATS_ALL=1 takes it for 16 too)
         if y.shape[-1] == 16 and os.environ.get("B200SEG_BWDSTATS_ALL", "0") != "1":
             return False
         dx, dy, da, df = _desc(x), _desc(y), _desc(addend), _desc(yfwd)

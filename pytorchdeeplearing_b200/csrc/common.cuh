@@ -1,4 +1,4 @@
-// Shared device/host helpers of the b200seg kernels (sm_100a only).
+// Shared device/host helpers of the b200seg kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -157,7 +157,7 @@ __device__ __forceinline__ void pdl_enter() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 #define PDL_ENTER() b200seg::pdl_enter()
-// Split form for kernels with an on-chip prologue (mbarrier init, TMEM allocation, shared-memory clears): trigger
+// Split form for kernels with an on-chip prologue (mbarrier init, shared-memory clears): trigger
 // first, run the prologue, THEN wait -- the prologue overlaps the tail of the kernel before.  Nothing before
 // PDL_WAIT() may touch global memory: a chain of triggered kernels can be resident before ANY of them has completed,
 // so not even data written many launches ago (packed weights) is safe to read early.  Every thread executes the wait.
@@ -195,10 +195,10 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
 
 inline int num_sms(int dev) {
   static int cached[64] = {0};
-  if (dev < 0 || dev >= 64) return 148;
+  if (dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     cached[dev] = v;
   }
   return cached[dev];

@@ -1,4 +1,4 @@
-// Generic implicit-GEMM convolution on CUDA cores (fp32 FFMA, fp32 accumulate) for sm_100a.
+// Generic implicit-GEMM convolution on CUDA cores (fp32 FFMA, fp32 accumulate) for sm_90a.
 //
 // Role (DESIGN.md section 4): (1) the whole conv family in PARITY mode (fp32 storage; fp32
 // products are what the 1e-3 / identical-argmax bar needs, SURVEY.md section 0.8), (2) in PERF

@@ -1,4 +1,4 @@
-// Halo-staged tcgen05 convolution for the full-resolution 16/32-channel 3x3(x3) layers (sm_100a, bf16).
+// Halo-staged wgmma convolution for the full-resolution 16/32-channel 3x3(x3) layers (sm_90a, bf16).
 //
 // conv_tc.cu loads one shifted activation box per tap through TMA: 27 L2->smem transfers of the same
 // voxels per output tile, which makes the 16/32-channel layers (80 % of the network's bytes) L2-bound.
@@ -7,15 +7,16 @@
 //     (18 x 10 voxels each, one-voxel halo, zero filled = conv padding) lives in smem, so each input voxel
 //     is fetched ~1.4x instead of 27x;
 //   * slices are stored channel-planar, [C/8 planes][18][10][8 ch], i.e. every voxel contributes one 16-byte
-//     K-chunk per plane and 8 consecutive voxels along w form one UMMA core matrix (8 rows x 16 B).  In the
+//     K-chunk per plane and 8 consecutive voxels along w form one wgmma core matrix (8 rows x 16 B).  In the
 //     no-swizzle K-major canonical layout the 16 core-matrix rows of the M = 128 tile are then a constant
 //     SBO = 160 B (one halo row) apart and the two K-chunks LBO = one plane apart, for EVERY tap: the tap only
 //     moves the descriptor start address by (kh*10 + kw)*16 B inside the slice selected by kd;
 //   * the packed weights of all taps stay resident in smem for the CTA's lifetime;
 //   * loader warps move global -> registers -> smem with 128-bit accesses (this is where norm-on-load will be
-//     fused); MMA issue, TMEM double buffering and the epilogue (bias, GroupNorm statistics, residual
-//     addend, bf16 NDHWC stores) follow conv_tc.cu.
-// Warp roles (416 threads): warp 0 MMA issuer + TMEM allocator, warps 1-4 epilogue, warps 5-12 loaders
+//     fused); the MMA warpgroup (two M64 halves, register accumulators), the double-buffered accumulator staging
+//     tile in shared memory and the epilogue (bias, GroupNorm statistics, residual addend, bf16 NDHWC stores)
+//     follow conv_tc.cu.
+// Warp roles (512 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue, warps 8-15 loaders
 // (software-pipelined: the loads of slice i+1 are in flight while slice i is stored).
 #include <stdlib.h>
 
@@ -27,7 +28,7 @@ constexpr int HT_W = 8, HT_H = 16;            // output tile (w, h); M = 128 row
 constexpr int HP_W = HT_W + 2, HP_H = HT_H + 2;
 constexpr int kHaloMaxSlices = 16;
 constexpr int kLoaderWarps = 8;
-constexpr int kHaloThreads = 32 * (1 + 4 + kLoaderWarps);
+constexpr int kHaloThreads = 32 * (4 + 4 + kLoaderWarps);
 constexpr int kMaxPieces = (HP_H * HP_W * 4 + 32 * kLoaderWarps - 1) / (32 * kLoaderWarps);   // Cin <= 32
 
 struct HaloArgs {
@@ -45,7 +46,7 @@ struct HaloArgs {
   int dchunk, ndchunks;   // output slices per work item, items along d
   int nitems;             // N * th * tw * ndchunks
   int nslices;            // ring size
-  int tmem_cols;
+  int acc_pitch;          // floats per row of the accumulator staging tile in shared memory
   int swap_lbo_sbo;       // debug: swap the roles of the two descriptor strides
   int cp_async;           // 1: loaders use cp.async (zfill) + mbarrier completion; 0: register-staged copies
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats): the output of this conv is
@@ -75,7 +76,7 @@ __device__ __forceinline__ void halo_stamp(const HaloArgs& p, int role, int idx)
 
 __device__ __forceinline__ uint64_t make_nosw_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) |
-         ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
+         ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 
 template <int CIN, int COUT, int KD>
@@ -96,8 +97,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
   uint64_t* sempty = sfull + kHaloMaxSlices;
   uint64_t* tfull = sempty + kHaloMaxSlices;
   uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* s_stat = reinterpret_cast<float*>(tmem_slot + 4);   // [4 epilogue warps][2][Cout]
+  float* s_stat = reinterpret_cast<float*>(tempty + 2);      // [4 epilogue warps][2][Cout]
+  float* s_acc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_stat + 8 * COUT) + 15) & ~(uintptr_t)15);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -110,24 +111,20 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
     for (int s = 0; s < p.nslices; ++s) {
       // register loader: one arrive per loader warp; cp.async loader: one (deferred) arrive per loader thread
       mbar_init(&sfull[s], p.cp_async ? 32 * kLoaderWarps : kLoaderWarps);
-      mbar_init(&sempty[s], 1);     // tcgen05.commit
+      mbar_init(&sempty[s], 4);     // one arrive per MMA warp
     }
     for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
+      mbar_init(&tfull[a], 4);
       mbar_init(&tempty[a], 4);
     }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   // resident weights: straight 16-byte copy of the pre-packed smem image
   for (uint32_t i = threadIdx.x * 16u; i < W_BYTES; i += blockDim.x * 16u)
     *reinterpret_cast<uint4*>(s_w + i) = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.w) + i);
   for (int i = threadIdx.x; i < 8 * p.Cout; i += blockDim.x) s_stat[i] = 0.f;
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   constexpr int pd = KD / 2;
 
   auto decode = [&](int item, int& n, int& h0, int& w0, int& d0, int& nd) {
@@ -142,9 +139,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
     nd = min(p.dchunk, p.D - d0);
   };
 
-  if (warp == 0) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(COUT >> 3) << 17) | ((128u >> 4) << 24);
+  if (warp < 4) {
+    // ===================================================== MMA warpgroup
+    const int wt = threadIdx.x;
     const uint32_t a_lbo = p.swap_lbo_sbo ? HP_W * 16u : PLANE;
     const uint32_t a_sbo = p.swap_lbo_sbo ? PLANE : HP_W * 16u;
     const uint32_t b_lbo = p.swap_lbo_sbo ? 128u : (uint32_t)COUT * 16u;
@@ -168,13 +165,17 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
           mbar_wait(&sfull[sl % p.nslices], (sl / p.nslices) & 1u);
         }
         const uint32_t as = go & 1u;
-        mbar_wait(&tempty[as], ((go >> 1) & 1u) ^ 1u);
         // slices written by cp.async (generic proxy) must be ordered before the tensor core's async-proxy reads
         fence_proxy_async();
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t tacc = tmem_base + as * (uint32_t)COUT;
-          // straight-line issue: every descriptor is (per-slice base) + compile-time offset, in 16-byte units
+        float acc0[COUT / 2], acc1[COUT / 2];
+        frag_zero(acc0);
+        frag_zero(acc1);
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        wgmma_fence();
+        {
+          // straight-line issue: every descriptor is (per-slice base) + compile-time offset, in 16-byte units;
+          // rows 64..127 of the tile (hh = 8..15) start 8 halo rows further on
 #pragma unroll
           for (int kd_ = 0; kd_ < KD; ++kd_) {
             const uint32_t sl = gs + o + kd_;
@@ -189,23 +190,34 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
                   (void)dummy;
                   const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)(kh_ * HP_W + kw_) * 16u) >> 4;
                   const uint32_t b_off = ((uint32_t)((((kd_ * 3 + kh_) * 3 + kw_) * kchunks + kc) * 2 * COUT) * 16u) >> 4;
-                  umma_bf16(tacc, a_base + a_off, b_base + b_off, idesc, (kd_ | kh_ | kw_ | kc) != 0 ? 1u : 0u);
+                  Wgmma<COUT, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
+                  Wgmma<COUT, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);
                 }
           }
-          umma_commit(&tfull[as]);
-          // input slice o is no longer needed; at the end of the item neither are the trailing KD-1
-          umma_commit(&sempty[(gs + o) % p.nslices]);
-          if (o == nd - 1)
-            for (int k = 1; k < KD; ++k) umma_commit(&sempty[(gs + o + k) % p.nslices]);
         }
+        wgmma_commit();
+        wgmma_wait0();
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
         __syncwarp();
+        if (lane == 0) {
+          // input slice o is no longer needed; at the end of the item neither are the trailing KD-1
+          mbar_arrive(&sempty[(gs + o) % p.nslices]);
+          if (o == nd - 1)
+            for (int k = 1; k < KD; ++k) mbar_arrive(&sempty[(gs + o + k) % p.nslices]);
+        }
+        mbar_wait(&tempty[as], ((go >> 1) & 1u) ^ 1u);
+        frag_store(s_acc + as * COUT, p.acc_pitch, 0, acc0, wt);
+        frag_store(s_acc + as * COUT, p.acc_pitch, 64, acc1, wt);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&tfull[as]);
       }
       gs += (uint32_t)nsl;
     }
-  } else if (warp >= 5) {
+  } else if (warp >= 8) {
     // ===================================================== loaders (8 warps, software pipelined)
     constexpr int LT = 32 * kLoaderWarps;
-    const int lt = threadIdx.x - 160;
+    const int lt = threadIdx.x - 256;
     const int pieces = HP_H * HP_W * CP;
     // this thread's pieces: q = lt + j*LT  ->  (voxel v, plane) -> smem offset and (hh, ww)
     int poff[kMaxPieces], phh[kMaxPieces], pww[kMaxPieces];
@@ -304,11 +316,11 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
     }
     }
   } else {
-    // ===================================================== epilogue warps 1..4
+    // ===================================================== epilogue warps 4..7
     const int q = warp & 3;
     const int row = q * 32 + lane;
     const int rw = row % HT_W, rh = row / HT_W;
-    const int etid = (warp - 1) * 32 + lane;
+    const int etid = (warp - 4) * 32 + lane;
     uint32_t go = 0;
     int cur_n = -1;
     auto flush_stats = [&](int n) {
@@ -340,11 +352,10 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
         const long long vox = (((long long)n * p.D + (d0 + o)) * p.H + oh) * p.W + ow;
         const uint32_t as = go & 1u;
         mbar_wait(&tfull[as], (go >> 1) & 1u);
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + as * (uint32_t)p.Cout + ((uint32_t)(q * 32) << 16);
+        const float* tacc = s_acc + row * p.acc_pitch + as * COUT;
         for (int c0 = 0; c0 < p.Cout; c0 += 16) {
           float v[16];
-          tmem_ld16(tacc + (uint32_t)c0, v);
+          acc_ld16(tacc + c0, v);
           if (p.bias != nullptr) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] += __ldg(p.bias + c0 + j);
@@ -391,19 +402,11 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
             store8(p.y + vox * p.yld + c0 + 8, v + 8);
           }
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) mbar_arrive(&tempty[as]);
       }
     }
     if (p.stats != nullptr && cur_n >= 0) flush_stats(cur_n);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -412,27 +415,54 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
 // Input-slice-major form of the 3-D kernel (KD = 3): every staged input slice is multiplied ONCE per (kh, kw, K chunk)
 // against the weights of all three kd taps side by side, B = [W(kd=2) | W(kd=1) | W(kd=0)] (N = 3*Cout columns), and
 // accumulates into the three output slices (i-2, i-1, i) it contributes to, which are neighbouring column ranges
-// of a TMEM ring of accumulators.  The M128 x N x K16 instruction is bound by the fetch of its A operand (128 voxel
-// rows re-read from shared memory per K step whatever N is: measured ~27 + 0.6*N cycles), so 9 instructions of
-// N = 3*Cout per input slice instead of 27 of N = Cout per output slice do the same MACs with a third of the A reads
-// (16 channels: 9 x ~57 instead of 27 x ~37 cycles per slice-tile; 32 channels: 18 x ~87 instead of 54 x ~47).
+// of a ring of accumulators.  An MMA instruction re-reads its A operand (the voxel rows) from shared memory whatever
+// N is, so 9 instructions of N = 3*Cout per input slice instead of 27 of N = Cout per output slice do the same MACs
+// with a third of the A reads.
 //   * accumulators: ring of kAccRing slots of Cout columns; slot of output o = (running output count) % ring; an
-//     output is complete when the input slice two further on has been issued (commit -> tfull[slot]);
-//   * all MMAs accumulate (the instruction-wide accumulate flag cannot distinguish the fresh third of its columns):
-//     the epilogue reads a slot into registers, hands it back ZEROED (tcgen05.st) at once and only then does its
-//     arithmetic; the whole ring is zeroed once at kernel start.  (Clearing a slot with an extra non-accumulating
-//     zero x zero MMA instead was measured: same time at 16 channels, 13 % slower at 32.)
+//     output is complete when the input slice two further on has been multiplied in (-> tfull[slot]);
+//   * all MMAs accumulate (one instruction spans the columns of up to three outputs): the epilogue reads a slot into
+//     registers, hands it back ZEROED at once and only then does its arithmetic; the whole ring is zeroed once at
+//     kernel start.
 //   * at the ends of an item's d-range the column range shrinks to the outputs that exist (N = Cout or 2*Cout,
 //     weight rows offset accordingly), and a range that would wrap around the ring is issued in two pieces;
 //   * the weight image in smem is the packed image permuted at load time to [(kh,kw)][Cin/8][kd reversed][Cout][8].
-// The per-slice chain of one CTA (barrier waits, MMA issue by a single thread, commits, TMEM read-and-zero) is latency
-// bound (tools/halo_timeline.py: ~460 ns of synchronisation + ~220 ns of MMA issue per slice, tensor pipe 15 % busy),
-// so the kernel is built to run TWO CTAs per SM: 288 threads (1 MMA issuer, 4 epilogue, 4 loader warps), <= 112 KB of
-// shared memory (4-8 slices), 128 / 256 TMEM columns, and the host splits d so that there are ~2 items per SM.
+// The accumulator ring lives in shared memory ([128 rows][ring * Cout] fp32): per input slice the MMA warpgroup
+// loads the columns of the outputs it contributes to into registers, runs the wgmma chain over them and stores them
+// back.  384 threads (4 MMA, 4 epilogue, 4 loader warps), one CTA per SM (two would leave 85 registers per thread).
 // ------------------------------------------------------------------------------------------------
-constexpr int kAccRing = 8;
-constexpr int kH3Loaders = 4;          // loader warps of the input-slice-major kernel (warps 5..8)
-constexpr int kH3Threads = 32 * (1 + 4 + kH3Loaders);   // 288 threads, TWO CTAs per SM
+constexpr int kAccRing = 4;
+constexpr int kH3Loaders = 4;          // loader warps of the input-slice-major kernel (warps 8..11)
+constexpr int kH3Threads = 32 * (4 + 4 + kH3Loaders);   // 384 threads
+
+// one contiguous piece of the accumulator ring (N = outputs x Cout columns starting at `acc`) += one staged input
+// slice x the (kh, kw) weights of the matching kd taps, for the whole MMA warpgroup (wt = thread index inside it)
+template <int CIN, int COUT, int N>
+__device__ __forceinline__ void halo3_mma(float* acc, int pitch, uint64_t a_base, uint64_t b_base, int wt) {
+  constexpr int CP = CIN / 8;
+  constexpr uint32_t PLANE = HP_H * HP_W * 16u;
+  constexpr int kchunks = CIN / 16;
+  float acc0[N / 2], acc1[N / 2];
+  frag_load(acc, pitch, 0, acc0, wt);
+  frag_load(acc, pitch, 64, acc1, wt);
+  wgmma_fence_regs(acc0);
+  wgmma_fence_regs(acc1);
+  wgmma_fence();
+#pragma unroll
+  for (int t9 = 0; t9 < 9; ++t9)
+#pragma unroll
+    for (int kc = 0; kc < kchunks; ++kc) {
+      const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)((t9 / 3) * HP_W + (t9 % 3)) * 16u) >> 4;
+      const uint32_t b_off = ((uint32_t)(t9 * CP + 2 * kc) * 3u * COUT * 16u) >> 4;
+      Wgmma<N, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
+      Wgmma<N, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);   // rows 64..127: hh 8..15
+    }
+  wgmma_commit();
+  wgmma_wait0();
+  wgmma_fence_regs(acc0);
+  wgmma_fence_regs(acc1);
+  frag_store(acc, pitch, 0, acc0, wt);
+  frag_store(acc, pitch, 64, acc1, wt);
+}
 constexpr int kHaloDepth = 6;          // cp.async groups (slices) in flight per loader thread; must be < ring slices
 
 template <int CIN, int COUT, int NCTA, bool BWD>
@@ -455,8 +485,7 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
   uint64_t* sempty = sfull + kHaloMaxSlices;
   uint64_t* tfull = sempty + kHaloMaxSlices;
   uint64_t* tempty = tfull + R;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + R);
-  float* s_stat = reinterpret_cast<float*>(tmem_slot + 4);   // [4 epilogue warps][2][Cout]
+  float* s_stat = reinterpret_cast<float*>(tempty + R);      // [4 epilogue warps][2][Cout]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -468,30 +497,23 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nslices; ++s) {
       mbar_init(&sfull[s], 1);                   // ONE arrive: by the loader warp that staged the slice
-      mbar_init(&sempty[s], 1);                  // tcgen05.commit
+      mbar_init(&sempty[s], 4);                  // one arrive per MMA warp
     }
     for (int a = 0; a < R; ++a) {
-      mbar_init(&tfull[a], 1);
+      mbar_init(&tfull[a], 4);
       mbar_init(&tempty[a], 4);
     }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   for (int i = threadIdx.x; i < 8 * p.Cout; i += blockDim.x) s_stat[i] = 0.f;
   float* s_bias = s_stat + 8 * COUT;
   float* s_ab = s_bias + COUT;                                       // [2][Cout]: A, B of the sample being processed
   double* s_gd = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(s_ab + 2 * COUT) + 7) & ~(uintptr_t)7);   // [2][Cout] + [8][2]
-  tc_fence_before();
+  float* s_acc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_gd + 2 * COUT + 16) + 15) & ~(uintptr_t)15);
+  // the accumulator ring starts at zero (every MMA accumulates)
+  for (int i = threadIdx.x; i < 128 * p.acc_pitch; i += blockDim.x) s_acc[i] = 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) halo_stamp(p, 0, 63);
-  if (warp >= 1 && warp <= 4) {
-    // the accumulator ring starts at zero (every MMA accumulates)
-    const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    for (int c = 0; c < R * COUT; c += 16) tmem_st16_zero(trow + (uint32_t)c);
-    tc_fence_before();
-  }
   // everything above is on-chip set-up and runs under the tail of the previous kernel; global memory from here on
   PDL_WAIT();
   // resident weights: 16-byte granules of the packed image [tap = (kd,kh,kw)][plane][co] -> [(kh,kw)][plane][2-kd][co]
@@ -507,7 +529,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
   for (int i = threadIdx.x; i < COUT; i += blockDim.x) s_bias[i] = p.bias != nullptr ? p.bias[i] : 0.f;
   fence_proxy_async();
   __syncthreads();
-  tc_fence_after();
   constexpr int pd = 1;
 
   auto decode = [&](int item, int& n, int& h0, int& w0, int& d0, int& nd) {
@@ -522,14 +543,13 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
     nd = min(p.dchunk, p.D - d0);
   };
 
-  if (warp == 0) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 4) << 24);   // | (N >> 3) << 17
+  if (warp < 4) {
+    // ===================================================== MMA warpgroup
+    const int wt = threadIdx.x;
     const uint64_t a_hi = make_nosw_desc(0, PLANE, HP_W * 16u);
     const uint64_t b_hi = make_nosw_desc(0, 3u * COUT * 16u, 128u);
     const uint32_t ring_u32 = smem_u32(s_ring);
     const uint32_t w_u32 = smem_u32(s_w);
-    constexpr int kchunks = CIN / 16;
     uint32_t gs = 0;   // input slices consumed so far (ring position of the item's first slice)
     uint32_t go = 0;   // output slices started so far (accumulator slot of the item's first output)
     for (int item = item_begin; item < item_end; ++item) {
@@ -539,7 +559,7 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
       for (int i = 0; i < nsl; ++i) {
         const uint32_t sl = gs + (uint32_t)i;
         mbar_wait(&sfull[sl % p.nslices], (sl / p.nslices) & 1u);
-        if (lane == 0) halo_stamp(p, 0, (int)sl);
+        if (wt == 0) halo_stamp(p, 0, (int)sl);
         if (i < nd) {
           // output i is touched for the first time: its slot must have been drained (and zeroed) by the epilogue
           const uint32_t gn_ = go + (uint32_t)i;
@@ -547,8 +567,7 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
         }
         // (the loader warp that staged the slice has waited for its cp.async group and executed
         //  fence.proxy.async BEFORE the arrive: the data is already ordered for the tensor core's async-proxy reads)
-        if (!(p.exp & 8)) tc_fence_after();
-        if (elect_one()) {
+        {
           const int lo = i - 2 > 0 ? i - 2 : 0;
           const int hi = i < nd - 1 ? i : nd - 1;
           const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % p.nslices) * SLICE) >> 4);
@@ -558,36 +577,33 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
             const uint32_t slot0 = (go + (uint32_t)o0) % R;
             int cnt = hi - o0 + 1;
             if ((int)slot0 + cnt > R) cnt = R - (int)slot0;
-            const uint32_t ncols = (uint32_t)cnt * COUT;
-            const uint32_t idesc = idesc0 | ((ncols >> 3) << 17);
-            const uint32_t tacc = tmem_base + slot0 * (uint32_t)COUT;
+            float* acc = s_acc + slot0 * COUT;
             const uint32_t row0 = (uint32_t)(2 - i + o0) * COUT;            // weight rows: kd = i - o  ->  (2 - kd) * Cout
             const uint64_t b_base = b_hi | (uint64_t)((w_u32 + row0 * 16u) >> 4);
-#pragma unroll
-            for (int t9 = 0; t9 < 9; ++t9)
-#pragma unroll
-              for (int kc = 0; kc < kchunks; ++kc) {
-                const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)((t9 / 3) * HP_W + (t9 % 3)) * 16u) >> 4;
-                const uint32_t b_off = ((uint32_t)(t9 * CP + 2 * kc) * 3u * COUT * 16u) >> 4;
-                if (!(p.exp & 1)) umma_bf16(tacc, a_base + a_off, b_base + b_off, idesc, 1u);
-              }
+            if (!(p.exp & 1)) {
+              if (cnt == 1) halo3_mma<CIN, COUT, COUT>(acc, p.acc_pitch, a_base, b_base, wt);
+              else if (cnt == 2) halo3_mma<CIN, COUT, 2 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
+              else halo3_mma<CIN, COUT, 3 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
+            }
             o0 += cnt;
           }
-          if (i >= 2) umma_commit(&tfull[(go + (uint32_t)(i - 2)) % R]);   // output i-2 has all three contributions
-          umma_commit(&sempty[sl % p.nslices]);                            // this input slice is consumed
-          halo_stamp(p, 1, (int)sl);
+          __syncwarp();
+          if (lane == 0) {
+            if (i >= 2) mbar_arrive(&tfull[(go + (uint32_t)(i - 2)) % R]);   // output i-2 has all three contributions
+            mbar_arrive(&sempty[sl % p.nslices]);                            // this input slice is consumed
+          }
+          if (wt == 0) halo_stamp(p, 1, (int)sl);
         }
-        __syncwarp();
       }
       gs += (uint32_t)nsl;
       go += (uint32_t)nd;
     }
-  } else if (warp >= 5) {
+  } else if (warp >= 8) {
     // ===================================================== loaders: 4 warps, warp w stages the input slices
     // sl = w (mod 4) on its own (all pieces of the slice, 16-byte cp.async with zero fill = conv padding), waits
     // for them to land and signals the slice with ONE mbarrier arrive.  The warps run independently: four slices
-    // are in flight per CTA, eight per SM (two CTAs are resident).
-    const int lw = warp - 5;
+    // are in flight per CTA.
+    const int lw = warp - 8;
     constexpr int pieces = HP_H * HP_W * CP;
     int it_item = item_begin, it_i = 0, it_nsl = 0, n = 0, h0 = 0, w0 = 0, d0 = 0, nd = 0;
     auto load_item = [&]() {
@@ -656,14 +672,14 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
       signal(prev_sl);
     }
   } else {
-    // ===================================================== epilogue warps 1..4
+    // ===================================================== epilogue warps 4..7
     // GroupNorm statistics: per-thread (= per output row) partial sums in registers over ALL slices of an item, one
-    // butterfly fold over the warp per item (not per slice); bias from shared memory; the zero hand-back of the
-    // accumulator columns is issued right after the read and only waited for before the slot is released.
+    // butterfly fold over the warp per item (not per slice); bias from shared memory; the accumulator columns are
+    // zeroed right after the read and the slot is released before the arithmetic.
     const int q = warp & 3;
     const int row = q * 32 + lane;
     const int rw = row % HT_W, rh = row / HT_W;
-    const int etid = (warp - 1) * 32 + lane;
+    const int etid = (warp - 4) * 32 + lane;
     uint32_t go = 0;
     int cur_n = -1;
     constexpr bool bwd = BWD;                 // backward-sums epilogue (b200seg_conv_bwdstats): its own instantiation,
@@ -755,24 +771,17 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
         }
         const uint32_t as = go % R;
         mbar_wait(&tfull[as], (go / R) & 1u);
-        tc_fence_after();
         if (etid == 0) halo_stamp(p, 3, (int)go);
-        const uint32_t tacc = tmem_base + as * (uint32_t)COUT + ((uint32_t)(q * 32) << 16);
+        float* tacc = s_acc + row * p.acc_pitch + as * COUT;
 #pragma unroll
         for (int c0 = 0; c0 < COUT; c0 += 16) {
           float v[16];
-          tmem_ld16(tacc + (uint32_t)c0, v);
-          {   // hand the columns back zeroed (all MMAs accumulate); completion is awaited before the release below
-            const uint32_t z = 0u;
-            asm volatile(
-                "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-                ::"r"(tacc + (uint32_t)c0), "r"(z)
-                : "memory");
-          }
+          acc_ld16(tacc + c0, v);
+#pragma unroll
+          for (int j = 0; j < 4; ++j)   // hand the columns back zeroed (all MMAs accumulate)
+            reinterpret_cast<float4*>(tacc + c0)[j] = make_float4(0.f, 0.f, 0.f, 0.f);
           if (c0 + 16 >= COUT) {
-            // every column of the slot is read and its zeroing issued: release it before the arithmetic
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
+            // every column of the slot is read and zeroed: release it before the arithmetic
             __syncwarp();
             if (lane == 0) mbar_arrive(&tempty[as]);
           }
@@ -873,7 +882,7 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
           qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
           if ((lane & 1) == 0) {
             const int col = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-            float* sw_ = s_stat + (warp - 1) * 2 * p.Cout;   // this warp's private row: no atomics, fixed order
+            float* sw_ = s_stat + (warp - 4) * 2 * p.Cout;   // this warp's private row: no atomics, fixed order
             sw_[c0 + col] += s[0];
             sw_[p.Cout + c0 + col] += qq[0];
           }
@@ -883,13 +892,8 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
     if (want_stats && cur_n >= 0) flush_stats(cur_n);
   }
 
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0) halo_stamp(p, 1, 63);
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -943,7 +947,7 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)); \
   B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm)); \
   B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100))
-    HALO3_ATTR(16, 16, 2); HALO3_ATTR(16, 32, 1); HALO3_ATTR(32, 16, 2); HALO3_ATTR(32, 32, 1);
+    HALO3_ATTR(16, 16, 1); HALO3_ATTR(16, 32, 1); HALO3_ATTR(32, 16, 1); HALO3_ATTR(32, 32, 1);
 #undef HALO3_ATTR
     g_halo_init[device] = 1;
   }
@@ -983,15 +987,14 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
     return (e && e[0] == '0') ? 0 : 1;            // input-slice-major kernel for the 3-D layers (default on)
   }();
   const bool use3 = halo3 && p.kd == 3;
-  // split d so that the grid covers the chip (each extra chunk re-loads kd-1 halo slices).  The input-slice-major
-  // kernel runs TWO CTAs per SM (and wants two items per SM) for 16 output channels; with 32 output channels the
-  // epilogue's register statistics do not fit the 96-register budget of two CTAs (and 32 -> 32 has 55 KB of weights):
-  // one CTA per SM with a deep ring (measured at 32 -> 32 @48^3: 30.7 us at one CTA, 34.8 us at two).
+  // split d so that the grid covers the chip (each extra chunk re-loads kd-1 halo slices); one CTA per SM with a
+  // deep slice ring
   const uint32_t slice = (uint32_t)(p.Cin / 8) * HP_H * HP_W * 16u;
   const uint32_t wbytes = ((uint32_t)(p.kd * 9) * p.Cin * p.Cout * 2u + 127u) & ~127u;
-  const uint32_t tail = (2 * kHaloMaxSlices + (use3 ? 2 * kAccRing : 4)) * 8 + 16 + (use3 ? 11 : 8) * p.Cout * 4 + 64 + (use3 ? (2 * p.Cout + 16) * 8 + 8 : 0);
-  const bool two = use3 && p.Cout == 16;       // 32 output channels: the epilogue's per-thread statistics need > 96 registers
-  const int slots = two ? 2 * sms : sms;
+  p.acc_pitch = (use3 ? kAccRing : 2) * p.Cout + 4;
+  const uint32_t tail = (2 * kHaloMaxSlices + (use3 ? 2 * kAccRing : 4)) * 8 + 16 + (use3 ? 11 : 8) * p.Cout * 4 + 64 +
+                        (use3 ? (2 * p.Cout + 16) * 8 + 8 : 0) + 16 + 128u * (uint32_t)p.acc_pitch * 4u;
+  const int slots = sms;
   int ndch = 1;
   if (cols < slots) {
     ndch = slots / cols;               // items <= slots: one item per CTA, no second wave
@@ -1001,14 +1004,11 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   p.dchunk = (p.D + ndch - 1) / ndch;
   p.ndchunks = (p.D + p.dchunk - 1) / p.dchunk;
   p.nitems = cols * p.ndchunks;
-  const int budget = two ? 112 * 1024 : maxsm;
+  const int budget = maxsm;
   int ns = (int)((budget - 256 - (int)wbytes - (int)tail) / (int)slice);
-  if (ns > (two ? 8 : kHaloMaxSlices)) ns = two ? 8 : kHaloMaxSlices;
+  if (ns > kHaloMaxSlices) ns = kHaloMaxSlices;
   B200_CHECK_ARG(ns >= p.kd + 1, "conv_halo: slices do not fit in shared memory");
   p.nslices = ns;
-  int tc = 32;
-  while (tc < (use3 ? kAccRing : 2) * p.Cout) tc *= 2;
-  p.tmem_cols = tc;
   static const int swap = [] {
     const char* e = getenv("B200SEG_HALO_SWAP");
     return (e && e[0] == '1') ? 1 : 0;
@@ -1044,9 +1044,9 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
     else launch_k(conv_halo3_kernel<CI, CO, NC, false>, grid, kH3Threads, smem_bytes, st, p);            \
   } while (0)
   if (use3) {
-    if (p.Cin == 16 && p.Cout == 16) HALO3_LAUNCH(16, 16, 2);
+    if (p.Cin == 16 && p.Cout == 16) HALO3_LAUNCH(16, 16, 1);
     else if (p.Cin == 16) HALO3_LAUNCH(16, 32, 1);
-    else if (p.Cout == 16) HALO3_LAUNCH(32, 16, 2);
+    else if (p.Cout == 16) HALO3_LAUNCH(32, 16, 1);
     else HALO3_LAUNCH(32, 32, 1);
   } else if (p.kd == 3) {
     if (p.Cin == 16 && p.Cout == 16) HALO_LAUNCH(16, 16, 3);

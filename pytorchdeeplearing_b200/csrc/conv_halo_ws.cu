@@ -1,4 +1,4 @@
-// Halo-staged tcgen05 3x3x3 convolution with STREAMED weights for the 64/128-channel pyramid levels (sm_100a, bf16).
+// Halo-staged wgmma 3x3x3 convolution with STREAMED weights for the 64/128-channel pyramid levels (sm_90a, bf16).
 //
 // At 24^3 / 12^3 voxels the TMA im2col path (conv_tc.cu) is bound by what one SM can ingest: every 128-voxel tile
 // pulls 27 shifted copies of its activation box plus all 27 tap blocks of the weights through L2->smem
@@ -9,11 +9,12 @@
 //   * weights: a work item covers NACC consecutive output slices of the column and NT output channels.  Each of the
 //     27 tap blocks ([Cin/8][NT][8] bf16, 4-8 KB) is streamed ONCE per item through a cp.async.bulk ring (as deep as
 //     the shared memory left over allows: the blocks in flight hide the L2 latency of the stream) and
-//     multiplied into all NACC accumulators (TMEM, NACC x NT columns, double buffered across items) before the
-//     next block is needed: weight traffic per tile drops by NACC, activation traffic by ~27 / (1 + 2/NACC).
+//     multiplied into all NACC accumulators (registers of the MMA warpgroup, NACC x NT columns) before the next
+//     block is needed: weight traffic per tile drops by NACC, activation traffic by ~27 / (1 + 2/NACC).  At the end
+//     of an item the accumulators go to a staging tile in shared memory (double buffered where it fits).
 // Items = samples x columns x ceil(D / NACC) x (Cout / NT), so even the 12^3 level spreads over ~100 CTAs.
-// Warp roles (448 threads): warp 0 MMA issuer + TMEM allocator, warps 1-4 epilogue (bias, GroupNorm statistics,
-// residual addend, bf16 NDHWC stores), warps 5-12 slice loaders (cp.async, zero fill), warp 13 weight streamer.
+// Warp roles (544 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue (bias, GroupNorm statistics, residual
+// addend, bf16 NDHWC stores), warps 8-15 slice loaders (cp.async, zero fill), warp 16 weight streamer.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -24,7 +25,7 @@ constexpr int WS_TW = 8, WS_TH = 16;                 // output tile (w, h); M = 
 constexpr int WS_PW = WS_TW + 2, WS_PH = WS_TH + 2;
 constexpr int kWsMaxSlices = 8;
 constexpr int kWsLoaderWarps = 8;
-constexpr int kWsThreads = 32 * (1 + 4 + kWsLoaderWarps + 1);
+constexpr int kWsThreads = 32 * (4 + 4 + kWsLoaderWarps + 1);
 constexpr int kWsMaxWStages = 16;     // weight ring depth is chosen at launch from the shared memory left over
 
 struct HaloWsArgs {
@@ -43,7 +44,8 @@ struct HaloWsArgs {
   int nitems;             // N * th * tw * ndchunks * ngroups
   int nslices;            // ring size (>= NACC + 2)
   int wstages;            // weight ring depth (tap blocks in flight)
-  int tmem_cols;
+  int accslots;           // accumulator staging slots in shared memory (1 or 2)
+  int acc_pitch;          // floats per staging row: accslots * NACC * NT + 4
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats; see conv_halo.cu)
   const bf16* yfwd;
   long long yfld;
@@ -66,7 +68,7 @@ __device__ __forceinline__ void ws_stamp(const HaloWsArgs& p, int slot) {
 }
 
 __device__ __forceinline__ uint64_t ws_nosw_desc(uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
+  return ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 
 template <int CIN, int NT, int NACC, bool BWD>
@@ -90,10 +92,10 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
   uint64_t* tempty = tfull + 2;
   uint64_t* wfull = tempty + 2;
   uint64_t* wempty = wfull + kWsMaxWStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wempty + kWsMaxWStages);
-  float* s_stat = reinterpret_cast<float*>(tmem_slot + 4);   // [4 epilogue warps][2][Cout]
+  float* s_stat = reinterpret_cast<float*>(wempty + kWsMaxWStages);   // [4 epilogue warps][2][Cout]
   float* s_ab = s_stat + 8 * p.Cout;                         // [2][Cout]: A, B of the sample being processed (BWD)
   double* s_gd = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(s_ab + 2 * p.Cout) + 7) & ~(uintptr_t)7);
+  float* s_acc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_gd + 2 * p.Cout + 16) + 15) & ~(uintptr_t)15);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -106,26 +108,22 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nslices; ++s) {
       mbar_init(&sfull[s], 32 * kWsLoaderWarps);     // one deferred cp.async arrive per loader thread
-      mbar_init(&sempty[s], 1);                      // tcgen05.commit
+      mbar_init(&sempty[s], 4);                      // one arrive per MMA warp
     }
     for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
+      mbar_init(&tfull[a], 4);
       mbar_init(&tempty[a], 4);
     }
     for (int a = 0; a < p.wstages; ++a) {
       mbar_init(&wfull[a], 1);
-      mbar_init(&wempty[a], 1);
+      mbar_init(&wempty[a], 4);
     }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   for (int i = threadIdx.x; i < 8 * p.Cout; i += blockDim.x) s_stat[i] = 0.f;
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  PDL_WAIT();               // barriers, TMEM and the statistics rows are set up under the tail of the previous kernel
+  PDL_WAIT();               // barriers and the statistics rows are set up under the tail of the previous kernel
   if (threadIdx.x == 0) ws_stamp(p, 1);
 
   // item -> (sample, column, first output slice, slices, channel group); the channel group is the fastest index
@@ -142,78 +140,103 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     nd = min(NACC, p.D - d0);
   };
 
-  if (warp == 0) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NT >> 3) << 17) | ((128u >> 4) << 24);
+  if (warp < 4) {
+    // ===================================================== MMA warpgroup
+    const int wt = threadIdx.x;
     const uint64_t a_hi = ws_nosw_desc(PLANE, WS_PW * 16u);
     const uint64_t b_hi = ws_nosw_desc((uint32_t)NT * 16u, 128u);
     const uint32_t ring_u32 = smem_u32(s_ring);
     const uint32_t w_u32 = smem_u32(s_w);
     constexpr int kchunks = CIN / 16;
     uint32_t gs = 0;    // slices consumed so far
-    uint32_t gi = 0;    // items done (accumulator set = gi & 1)
+    uint32_t gi = 0;    // items done (accumulator slot = gi % accslots)
     uint32_t wst = 0;   // weight blocks consumed so far
     for (int item = item_begin; item < item_end; ++item, ++gi) {
       int n, h0, w0, d0, nd, ng;
       decode(item, n, h0, w0, d0, nd, ng);
       const int nsl = nd + 2;
-      const uint32_t as = gi & 1u;
-      mbar_wait(&tempty[as], ((gi >> 1) & 1u) ^ 1u);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t tacc = tmem_base + as * (uint32_t)(NACC * NT);
-        // slices are waited for when first needed: kd = 0 touches slices 0..nd-1, every further kd one more,
-        // so the multiplications start while the tail of the item's slices is still in flight
-        auto wait_slice = [&](int k) {
-          const uint32_t sl = gs + (uint32_t)k;
-          mbar_wait(&sfull[sl % (uint32_t)p.nslices], (sl / (uint32_t)p.nslices) & 1u);
-        };
+      const uint32_t as = gi % (uint32_t)p.accslots;
+      float acc0[NACC][NT / 2], acc1[NACC][NT / 2];
 #pragma unroll
-        for (int kd_ = 0; kd_ < 3; ++kd_) {
-          if (kd_ == 0) {
-            for (int k = 0; k < nd; ++k) wait_slice(k);
-            if (gi == 0) ws_stamp(p, 2);
-          } else {
-            wait_slice(nd - 1 + kd_);
-          }
-          fence_proxy_async();      // cp.async (generic proxy) writes -> tensor core (async proxy) reads
+      for (int j = 0; j < NACC; ++j) {
+        frag_zero(acc0[j]);
+        frag_zero(acc1[j]);
+      }
+      // slices are waited for when first needed: kd = 0 touches slices 0..nd-1, every further kd one more,
+      // so the multiplications start while the tail of the item's slices is still in flight
+      auto wait_slice = [&](int k) {
+        const uint32_t sl = gs + (uint32_t)k;
+        mbar_wait(&sfull[sl % (uint32_t)p.nslices], (sl / (uint32_t)p.nslices) & 1u);
+      };
 #pragma unroll
-          for (int kh_ = 0; kh_ < 3; ++kh_)
+      for (int kd_ = 0; kd_ < 3; ++kd_) {
+        if (kd_ == 0) {
+          for (int k = 0; k < nd; ++k) wait_slice(k);
+          if (gi == 0 && wt == 0) ws_stamp(p, 2);
+        } else {
+          wait_slice(nd - 1 + kd_);
+        }
+        fence_proxy_async();      // cp.async (generic proxy) writes -> tensor core (async proxy) reads
 #pragma unroll
-            for (int kw_ = 0; kw_ < 3; ++kw_) {
-              const uint32_t wq = wst + (uint32_t)((kd_ * 3 + kh_) * 3 + kw_);
-              const uint32_t stg = wq % (uint32_t)p.wstages;
-              mbar_wait(&wfull[stg], (wq / (uint32_t)p.wstages) & 1u);
-              tc_fence_after();
-              const uint64_t b_tap = b_hi | (uint64_t)((w_u32 + stg * TAP_BYTES) >> 4);
+        for (int kh_ = 0; kh_ < 3; ++kh_)
 #pragma unroll
-              for (int j = 0; j < NACC; ++j) {
-                if (j < nd) {
-                  const uint32_t sl = gs + (uint32_t)(j + kd_);
-                  const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % (uint32_t)p.nslices) * SLICE) >> 4);
+          for (int kw_ = 0; kw_ < 3; ++kw_) {
+            const uint32_t wq = wst + (uint32_t)((kd_ * 3 + kh_) * 3 + kw_);
+            const uint32_t stg = wq % (uint32_t)p.wstages;
+            mbar_wait(&wfull[stg], (wq / (uint32_t)p.wstages) & 1u);
+            const uint64_t b_tap = b_hi | (uint64_t)((w_u32 + stg * TAP_BYTES) >> 4);
 #pragma unroll
-                  for (int kc = 0; kc < kchunks; ++kc) {
-                    const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)(kh_ * WS_PW + kw_) * 16u) >> 4;
-                    const uint32_t b_off = ((uint32_t)(kc * 2 * NT) * 16u) >> 4;
-                    umma_bf16(tacc + (uint32_t)(j * NT), a_base + a_off, b_tap + b_off, idesc,
-                              (kd_ | kh_ | kw_ | kc) != 0 ? 1u : 0u);
-                  }
+            for (int j = 0; j < NACC; ++j) {
+              wgmma_fence_regs(acc0[j]);
+              wgmma_fence_regs(acc1[j]);
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < NACC; ++j) {
+              if (NACC == 1 || j < nd) {
+                const uint32_t sl = gs + (uint32_t)(j + kd_);
+                const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % (uint32_t)p.nslices) * SLICE) >> 4);
+#pragma unroll
+                for (int kc = 0; kc < kchunks; ++kc) {
+                  const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)(kh_ * WS_PW + kw_) * 16u) >> 4;
+                  const uint32_t b_off = ((uint32_t)(kc * 2 * NT) * 16u) >> 4;
+                  Wgmma<NT, 0, 0>::mma(acc0[j], a_base + a_off, b_tap + b_off);
+                  // rows 64..127 of the tile (hh = 8..15) start 8 halo rows further on
+                  Wgmma<NT, 0, 0>::mma(acc1[j], a_base + a_off + (8u * WS_PW * 16u >> 4), b_tap + b_off);
                 }
               }
-              umma_commit(&wempty[stg]);
             }
-        }
-        if (gi == 0) ws_stamp(p, 3);
-        umma_commit(&tfull[as]);
+            wgmma_commit();
+            wgmma_wait0();
+#pragma unroll
+            for (int j = 0; j < NACC; ++j) {
+              wgmma_fence_regs(acc0[j]);
+              wgmma_fence_regs(acc1[j]);
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&wempty[stg]);
+          }
+      }
+      if (gi == 0 && wt == 0) ws_stamp(p, 3);
+      __syncwarp();
+      if (lane == 0) {
 #pragma unroll
         for (int k = 0; k < NSL; ++k)
-          if (k < nsl) umma_commit(&sempty[(gs + (uint32_t)k) % (uint32_t)p.nslices]);
+          if (k < nsl) mbar_arrive(&sempty[(gs + (uint32_t)k) % (uint32_t)p.nslices]);
+      }
+      mbar_wait(&tempty[as], ((gi / (uint32_t)p.accslots) & 1u) ^ 1u);
+#pragma unroll
+      for (int j = 0; j < NACC; ++j) {
+        float* acc = s_acc + as * (uint32_t)(NACC * NT) + j * NT;
+        frag_store(acc, p.acc_pitch, 0, acc0[j], wt);
+        frag_store(acc, p.acc_pitch, 64, acc1[j], wt);
       }
       __syncwarp();
+      if (lane == 0) mbar_arrive(&tfull[as]);
       gs += (uint32_t)nsl;
       wst += TAPS;
     }
-  } else if (warp == 5 + kWsLoaderWarps) {
+  } else if (warp == 8 + kWsLoaderWarps) {
     // ===================================================== weight streamer: tap blocks -> ring (one lane)
     if (lane == 0) {
       uint32_t wst = 0;
@@ -233,10 +256,10 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
         }
       }
     }
-  } else if (warp >= 5) {
+  } else if (warp >= 8) {
     // ===================================================== slice loaders (8 warps, cp.async with zero fill)
     constexpr int LT = 32 * kWsLoaderWarps;
-    const int lt = threadIdx.x - 160;
+    const int lt = threadIdx.x - 256;
     const int pieces = WS_PH * WS_PW * CP;
     int poff[kMaxPieces], phh[kMaxPieces], pww[kMaxPieces];
     bool pval[kMaxPieces];
@@ -278,11 +301,11 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
   } else {
-    // ===================================================== epilogue warps 1..4
+    // ===================================================== epilogue warps 4..7
     const int q = warp & 3;
     const int row = q * 32 + lane;
     const int rw = row % WS_TW, rh = row / WS_TW;
-    const int etid = (warp - 1) * 32 + lane;
+    const int etid = (warp - 4) * 32 + lane;
     uint32_t gi = 0;
     int cur_n = -1;
     auto flush_stats = [&](int n) {
@@ -344,11 +367,10 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       const int oh = h0 + rh, ow = w0 + rw;
       const bool valid = oh < p.H && ow < p.W;
       const int cbase = ng * NT;
-      const uint32_t as = gi & 1u;
-      mbar_wait(&tfull[as], (gi >> 1) & 1u);
-      tc_fence_after();
+      const uint32_t as = gi % (uint32_t)p.accslots;
+      mbar_wait(&tfull[as], (gi / (uint32_t)p.accslots) & 1u);
       if (etid == 0 && gi == 0) ws_stamp(p, 4);
-      const uint32_t tacc = tmem_base + as * (uint32_t)(NACC * NT) + ((uint32_t)(q * 32) << 16);
+      const float* tacc = s_acc + row * p.acc_pitch + as * (NACC * NT);
       // GroupNorm statistics: per-thread (row) partials over the item's tiles, ONE warp fold per 16-column chunk
       // and item (chunk-outer order keeps only one chunk's partials in registers)
 #pragma unroll 1
@@ -371,7 +393,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
             }
           }
           float v[16];
-          tmem_ld16(tacc + (uint32_t)(o * NT + c * 16), v);
+          acc_ld16(tacc + o * NT + c * 16, v);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             v[j] += bv[j];
@@ -426,7 +448,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
         if (c == NT / 16 - 1) {
           // the accumulators are drained: hand them back before the last (register-only) statistics fold
           if (etid == 0 && gi == 0) ws_stamp(p, 5);
-          tc_fence_before();
           __syncwarp();
           if (lane == 0) mbar_arrive(&tempty[as]);
         }
@@ -458,13 +479,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     if (p.stats != nullptr && cur_n >= 0) flush_stats(cur_n);
   }
 
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0) ws_stamp(p, 6);
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -497,12 +513,19 @@ static int conv_halows_launch(HaloWsArgs& p, int device, int maxsm, cudaStream_t
   // (tail: + A/B table and its fp64 scratch for the backward-sums epilogue)
   const uint32_t slice = (uint32_t)(CIN / 8) * WS_PH * WS_PW * 16u;
   const uint32_t tap_bytes = (uint32_t)CIN * NT * 2u;
-  const uint32_t tail = (2 * kWsMaxSlices + 4 + 2 * kWsMaxWStages) * 8 + 16 + 10 * p.Cout * 4 + 64 +
-                        (2 * p.Cout + 16) * 8 + 8;
-  // one item's slices stay resident; everything left goes to the weight ring (tap blocks in flight hide the
-  // L2 latency of the stream: each block is consumed in ~0.1 us)
+  const uint32_t tail0 = (2 * kWsMaxSlices + 4 + 2 * kWsMaxWStages) * 8 + 16 + 10 * p.Cout * 4 + 64 +
+                         (2 * p.Cout + 16) * 8 + 8 + 16;
+  // one item's slices stay resident; the staging tile is double buffered if four weight blocks still fit beside it;
+  // the rest is the weight ring (tap blocks in flight hide the L2 latency of the stream)
   const int ns = NACC + 2;
-  int wst = (maxsm - 256 - (int)tail - ns * (int)slice) / (int)tap_bytes;
+  int wst = 0;
+  uint32_t tail = 0;
+  for (p.accslots = 2; p.accslots >= 1; --p.accslots) {
+    p.acc_pitch = p.accslots * NACC * NT + 4;
+    tail = tail0 + 128u * (uint32_t)p.acc_pitch * 4u;
+    wst = (maxsm - 256 - (int)tail - ns * (int)slice) / (int)tap_bytes;
+    if (wst >= 4 || p.accslots == 1) break;
+  }
   if (wst > kWsMaxWStages) wst = kWsMaxWStages;
   B200_CHECK_ARG(wst >= 2, "conv_halows: slices do not fit in shared memory");
   p.nslices = ns;
@@ -511,9 +534,6 @@ static int conv_halows_launch(HaloWsArgs& p, int device, int maxsm, cudaStream_t
   p.ndchunks = (p.D + NACC - 1) / NACC;
   p.ngroups = p.Cout / NT;
   p.nitems = p.N * p.th * p.tw * p.ndchunks * p.ngroups;
-  int tc = 32;
-  while (tc < 2 * NACC * NT) tc *= 2;
-  p.tmem_cols = tc;
   const size_t smem_bytes = 128 + wbytes + (size_t)ns * slice + tail;
   const int sms = num_sms(device);
   const int grid = sms < p.nitems ? sms : p.nitems;
@@ -529,9 +549,9 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
   (void)kind; (void)dims;
   const int maxsm = tc_max_smem(device);
   if (device >= 0 && device < 64 && !g_ws_init[device]) {
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
     B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<128, 64, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
     B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<128, 64, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
     g_ws_init[device] = 1;
   }
@@ -567,10 +587,9 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
     const char* e = getenv("B200SEG_WS_DBG");
     p.dbg = e ? reinterpret_cast<unsigned long long*>(strtoull(e, nullptr, 16)) : nullptr;
   }
-  // NT = 64 columns per MMA (an SS-mode MMA is paced by reading its 128-row A operand from shared memory, ~50
-  // cycles per K = 16 step whatever N is, so narrow column groups waste the tensor core); NACC is then chosen so
-  // that the level still yields ~100-150 work items
-  if (p.Cin == 64) return conv_halows_launch<64, 64, 2>(p, device, maxsm, st);
+  // NT = 64 columns per MMA (narrower groups re-read A for less work); NACC = 1 keeps the warpgroup at 64
+  // accumulator registers per thread, within the budget of a 544-thread CTA
+  if (p.Cin == 64) return conv_halows_launch<64, 64, 1>(p, device, maxsm, st);
   return conv_halows_launch<128, 64, 1>(p, device, maxsm, st);
 }
 

@@ -1,4 +1,4 @@
-// tcgen05 + TMA implicit-GEMM convolution for sm_100a (bf16 operands, fp32 accumulation in TMEM).
+// wgmma + TMA implicit-GEMM convolution for sm_90a (bf16 operands, fp32 accumulation in registers).
 //
 // Covers the dense-MMA-shaped members of the conv family in PERF mode: 3x3x3 / 3x3 (pad 1) and
 // 1x1x1 convolutions, forward and data-gradient form, Cin in {16, 32, 64k}, Cout = 16..256 (x16).
@@ -7,14 +7,15 @@
 // K = taps x Cin.  One pipeline stage = one tap x one 16/32/64-channel block:
 //   A tile  : TMA 5-D tiled load of the NDHWC activation box shifted by the tap offset; the
 //             hardware zero-fills out-of-bounds voxels = the conv's zero padding; 128 rows of
-//             BKC*2 bytes land K-major with the 32/64/128-byte swizzle the UMMA descriptor names.
+//             BKC*2 bytes land K-major with the 32/64/128-byte swizzle the wgmma descriptor names.
 //   B tile  : TMA 2-D load of the [tap*Cout + co][ci] packed weights (K-major, same swizzle).
-//   MMA     : one elected thread issues BKC/16 tcgen05.mma (M128 x N x K16) per stage into a TMEM
-//             accumulator; tcgen05.commit releases the smem stage / publishes the accumulator.
-// Warp roles (320 threads): warp 0 TMA producer, warp 1 TMEM allocator + MMA issuer, warps 2-9 epilogue in two groups
-// of four (one warp per TMEM lane quarter; group e drains the tiles with local index = e mod 2):
-// tcgen05.ld -> +bias -> GroupNorm sum/sumsq partials -> +addend -> bf16 NDHWC stores.
-// Up to four accumulator stages in TMEM let the MMA issuer run ahead of the epilogue; CTAs are persistent over
+//   MMA     : the MMA warpgroup issues 2 x BKC/16 wgmma (two M64 halves x N x K16) per stage into register
+//             accumulators (N <= 64), then releases the smem stage; at the end of the K loop it writes the
+//             accumulator tile to one of two fp32 staging slots in shared memory and publishes it.
+// Warp roles (512 threads): warp 0 TMA producer, warps 1-3 idle, warps 4-7 MMA warpgroup, warps 8-15 epilogue in two
+// groups of four (group e drains the tiles with local index = e mod 2, one thread per tile row):
+// staged accumulator row -> +bias -> GroupNorm sum/sumsq partials -> +addend -> bf16 NDHWC stores.
+// The two staging slots let the MMA warpgroup run one tile ahead of each epilogue group; CTAs are persistent over
 // contiguous tile ranges (grid = min(tiles, #SM)).
 #include <stdlib.h>
 
@@ -62,8 +63,8 @@ struct TcArgs {
   int tw, th, td;         // tiles per dim
   int ntiles;             // N * td * th * tw
   int nstages;
-  int nacc;               // accumulator stages in TMEM (2 or 4)
-  int tmem_cols;          // power of two >= nacc*Ntile (>= 32)
+  int nacc;               // accumulator staging slots in shared memory (== kMaxAcc)
+  int acc_pitch;          // floats per row of the staging tile: nacc*Ntile + 4
   // split-K (deep, small levels): the (tap, channel-block) loop of one (voxel tile, column group) is cut into
   // `ksplit` ranges, one work item each; every item leaves its fp32 partial in its own slab of `ws`, and the item
   // that arrives last (counted in cnt[tile, group]) adds the slabs in split order and runs the usual epilogue
@@ -73,10 +74,11 @@ struct TcArgs {
 };
 
 constexpr int kMaxStages = 8;
-constexpr int kEpiWarps = 4;          // warps per epilogue group (one per TMEM lane quarter)
-constexpr int kEpiGroups = 2;         // group e drains accumulator stage e: two tiles are in the epilogue at a time
-constexpr int kTcThreads = 64 + 32 * kEpiWarps * kEpiGroups;
-constexpr int kMaxAcc = 4;            // TMEM accumulator stages (the MMA issuer runs this many tiles ahead of the epilogue)
+constexpr int kEpiWarps = 4;          // warps per epilogue group (32 tile rows each)
+constexpr int kEpiGroups = 2;         // group e drains accumulator slot e: two tiles are in the epilogue at a time
+constexpr int kTcThreads = 256 + 32 * kEpiWarps * kEpiGroups;
+constexpr int kMaxAcc = 2;            // accumulator staging slots (one per epilogue group)
+constexpr int kTcMaxN = 64;           // MMA N per tile: both M64 halves of the accumulator stay in registers
 
 // butterfly transpose-reduce of 16 per-lane column values (and their squares) over the 32 lanes of a warp:
 // afterwards every EVEN lane L holds in s[0] / q[0] the warp totals of column stat_col(L)
@@ -102,6 +104,58 @@ __device__ __forceinline__ int stat_col(int lane) {
   return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
 }
 
+template <int BKC, int N>
+__device__ __forceinline__ void tc_mma_role(const TcArgs& p, const uint8_t* smem, uint32_t STAGE, uint64_t* full,
+                                            uint64_t* empty, uint64_t* tfull, uint64_t* tempty, float* s_acc,
+                                            int tile_begin, int tile_end, int kblocks, int wt) {
+  constexpr uint32_t SWZ = BKC * 2;
+  constexpr uint32_t A_BYTES = 128u * SWZ;
+  constexpr int R = N / 2;
+  const int S = p.ksplit;
+  const int lane = wt & 31;
+  uint32_t it = 0;
+  int local = 0;
+  for (int item = tile_begin; item < tile_end; ++item, ++local) {
+    const uint32_t as = (uint32_t)local % (uint32_t)p.nacc;
+    const uint32_t aph = ((uint32_t)local / (uint32_t)p.nacc) & 1u;
+    float d0[R], d1[R];
+    frag_zero(d0);
+    frag_zero(d1);
+    const int sp = item % S;
+    const int kb0 = sp * kblocks / S, kb1 = (sp + 1) * kblocks / S;
+    for (int kb = kb0; kb < kb1; ++kb, ++it) {
+      const uint32_t s = it % p.nstages;
+      const uint32_t ph = (it / p.nstages) & 1u;
+      mbar_wait(&full[s], ph);
+      const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
+      const uint64_t adesc = make_kmajor_desc(sa, SWZ);
+      const uint64_t bdesc = make_kmajor_desc(sa + A_BYTES, SWZ);
+      wgmma_fence_regs(d0);
+      wgmma_fence_regs(d1);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BKC / 16; ++k) {
+        // +32 bytes (2 x 16-byte units) per K=16 step inside the swizzle atom; rows 64..127 start 64 rows further on
+        Wgmma<N, 0, 0>::mma(d0, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+        Wgmma<N, 0, 0>::mma(d1, adesc + (uint64_t)((64u * SWZ) >> 4) + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k));
+      }
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_fence_regs(d0);
+      wgmma_fence_regs(d1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    // the epilogue group of this slot has drained the previous tile
+    mbar_wait(&tempty[as], aph ^ 1u);
+    float* acc = s_acc + as * N;
+    frag_store(acc, p.acc_pitch, 0, d0, wt);
+    frag_store(acc, p.acc_pitch, 64, d1, wt);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&tfull[as]);
+  }
+}
+
 // NCH > 0 (Cout == 16 * NCH <= 32): the layers with few MACs per output element (1x1x1, 2x2x2 stride 2 and its
 // transpose at 16/32 channels) are bound by the epilogue, so their GroupNorm statistics are accumulated per
 // thread in registers across all of the CTA's tiles and folded over the warp once per sample, and the bias lives
@@ -122,9 +176,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   uint64_t* empty = full + kMaxStages;
   uint64_t* tfull = empty + kMaxStages;
   uint64_t* tempty = tfull + kMaxAcc;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + kMaxAcc);
-  float* s_stat = reinterpret_cast<float*>(tmem_slot + 4);     // [2 groups][4 epilogue warps][2][Cout]
+  float* s_stat = reinterpret_cast<float*>(tempty + kMaxAcc);  // [2 groups][4 epilogue warps][2][Cout]
   unsigned int* s_flag = reinterpret_cast<unsigned int*>(s_stat + 8 * kEpiGroups * p.Cout);   // [2 groups]
+  float* s_acc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_flag + kEpiGroups) + 15) & ~(uintptr_t)15);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -142,10 +196,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nstages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 4);      // one arrive per MMA warp
     }
     for (int a = 0; a < kMaxAcc; ++a) {
-      mbar_init(&tfull[a], 1);
+      mbar_init(&tfull[a], 4);
       mbar_init(&tempty[a], kEpiWarps);
     }
     fence_barrier_init();
@@ -154,12 +208,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   for (int i = threadIdx.x; i < 8 * kEpiGroups * p.Cout; i += blockDim.x) s_stat[i] = 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   PDL_WAIT();               // everything above is on-chip set-up: it runs under the tail of the previous kernel
 
   if (warp == 0) {
@@ -194,49 +244,24 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.Ntile >> 3) << 17) | ((128u >> 4) << 24);
-    uint32_t it = 0;
-    int local = 0;
-    for (int item = tile_begin; item < tile_end; ++item, ++local) {
-      const uint32_t as = (uint32_t)local % (uint32_t)p.nacc;
-      const uint32_t aph = ((uint32_t)local / (uint32_t)p.nacc) & 1u;
-      mbar_wait(&tempty[as], aph ^ 1u);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + as * (uint32_t)p.Ntile;
-      const int sp = item % S;
-      const int kb0 = sp * kblocks / S, kb1 = (sp + 1) * kblocks / S;
-      for (int kb = kb0; kb < kb1; ++kb, ++it) {
-        const uint32_t s = it % p.nstages;
-        const uint32_t ph = (it / p.nstages) & 1u;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
-          const uint64_t adesc = make_kmajor_desc(sa, SWZ);
-          const uint64_t bdesc = make_kmajor_desc(sa + A_BYTES, SWZ);
-#pragma unroll
-          for (int k = 0; k < BKC / 16; ++k) {
-            // +32 bytes (2 x 16-byte units) per K=16 step inside the swizzle atom
-            umma_bf16(tacc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                      (kb != kb0 || k != 0) ? 1u : 0u);
-          }
-          umma_commit(&empty[s]);
-          if (kb == kb1 - 1) umma_commit(&tfull[as]);
-        }
-        __syncwarp();
-      }
+  } else if (warp >= 4 && warp < 8) {
+    // ===================================================== MMA warpgroup
+    const int wt = threadIdx.x - 128;
+    switch (p.Ntile) {
+      case 16: tc_mma_role<BKC, 16>(p, smem, STAGE, full, empty, tfull, tempty, s_acc, tile_begin, tile_end, kblocks, wt); break;
+      case 32: tc_mma_role<BKC, 32>(p, smem, STAGE, full, empty, tfull, tempty, s_acc, tile_begin, tile_end, kblocks, wt); break;
+      case 48: tc_mma_role<BKC, 48>(p, smem, STAGE, full, empty, tfull, tempty, s_acc, tile_begin, tile_end, kblocks, wt); break;
+      default: tc_mma_role<BKC, 64>(p, smem, STAGE, full, empty, tfull, tempty, s_acc, tile_begin, tile_end, kblocks, wt); break;
     }
-  } else {
-    // ===================================================== epilogue warps (2..9), two groups of four
-    const int eg = (warp - 2) >> 2;               // group = accumulator stage it drains
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
+  } else if (warp >= 8) {
+    // ===================================================== epilogue warps (8..15), two groups of four
+    const int eg = (warp - 8) >> 2;               // group = accumulator slot it drains
+    const int q = warp & 3;                       // quarter of the tile rows this warp handles
     const int row = q * 32 + lane;                // row of the M tile = voxel of the box
     const int rw = row % p.bw;
     const int rh = (row / p.bw) % p.bh;
     const int rd = row / (p.bw * p.bh);
-    const int etid = (threadIdx.x - 64) & 127;    // 0..127 inside the group
+    const int etid = (threadIdx.x - 256) & 127;   // 0..127 inside the group
     float* s_stat_g = s_stat + eg * 8 * p.Cout;   // [4 warps][2][Cout] of this group
     int cur_n = -1;
     constexpr int NR = NCH > 0 ? NCH : 1;
@@ -296,20 +321,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       const uint32_t as = (uint32_t)local % (uint32_t)p.nacc;
       const uint32_t aph = ((uint32_t)local / (uint32_t)p.nacc) & 1u;
       mbar_wait(&tfull[as], aph);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + as * (uint32_t)p.Ntile + ((uint32_t)(q * 32) << 16);
+      const float* tacc = s_acc + row * p.acc_pitch + as * p.Ntile;
       const float4* slabs = nullptr;
       if (S > 1) {
         // partial sums of this K range -> own slab; the accumulator is free as soon as it has been read
         float4* mine = p.ws + ((size_t)tg * S + sp) * (size_t)(p.Ntile / 4) * 128 + row;
         for (int cc = 0; cc < p.Ntile; cc += 16) {
           float v[16];
-          tmem_ld16(tacc + (uint32_t)cc, v);
+          acc_ld16(tacc + cc, v);
 #pragma unroll
           for (int j = 0; j < 4; ++j)
             __stcg(mine + (size_t)(cc / 4 + j) * 128, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) mbar_arrive(&tempty[as]);
         __threadfence();
@@ -328,7 +351,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
       for (int cc = 0; cc < p.Ntile; cc += 16) {
         float v[16];
         if (S == 1) {
-          tmem_ld16(tacc + (uint32_t)cc, v);
+          acc_ld16(tacc + cc, v);
         } else {
           // fixed order over the K ranges: the result does not depend on which range finished last
 #pragma unroll
@@ -402,19 +425,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) conv_tc_kernel(const __grid_con
         }
       }
       if (S == 1) {
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) mbar_arrive(&tempty[as]);
       }
     }
     if (p.stats != nullptr && cur_n >= 0) flush_stats(cur_n);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -558,7 +573,8 @@ int conv_tc(int kind, int dims, const b200seg_tensor* x, const void* wpk, const 
   p.sd = g.sd; p.sh = g.sh; p.sw = g.sw;
   p.up = g.up; p.ud = g.ud; p.uh = g.uh; p.uw = g.uw;
   const int ncols = g.up ? g.ud * g.uh * g.uw * p.Cout : p.Cout;
-  p.Ntile = ncols > 256 ? 256 : ncols;
+  p.Ntile = kTcMaxN;
+  while (ncols % p.Ntile) p.Ntile -= 16;       // widest column group (multiple of 16, <= 64) that divides the columns
   p.ngroups = ncols / p.Ntile;
   p.ksplit = 1;
   p.ws = nullptr;
@@ -606,16 +622,16 @@ int conv_tc(int kind, int dims, const b200seg_tensor* x, const void* wpk, const 
   const uint32_t a_bytes = 128u * swz;
   const uint32_t b_bytes = (((uint32_t)p.Ntile * swz) + 1023u) & ~1023u;
   const uint32_t stage = a_bytes + b_bytes;
-  const uint32_t tail = (2 * kMaxStages + 2 * kMaxAcc) * 8 + 16 + 8 * kEpiGroups * p.Cout * 4 + 16;
+  // barriers, statistics rows, flags and the accumulator staging tile (128 rows of nacc*Ntile + 4 floats)
+  const uint32_t tail = (2 * kMaxStages + 2 * kMaxAcc) * 8 + 8 * kEpiGroups * p.Cout * 4 + 16 + 16 +
+                        128u * (uint32_t)(kMaxAcc * p.Ntile + 4) * 4u;
   const int maxsm = g_smem_optin[device] > 0 ? g_smem_optin[device] : 227 * 1024;
   int nst = (int)((maxsm - 1024 - (int)tail - 256) / (int)stage);
   if (nst > kMaxStages) nst = kMaxStages;
   B200_CHECK_ARG(nst >= 2, "conv_tc: tile does not fit in shared memory (Cin=%d Cout=%d)", p.Cin, p.Cout);
   p.nstages = nst;
-  p.nacc = p.Ntile * kMaxAcc <= 512 ? kMaxAcc : 2;
-  int cols = 32;
-  while (cols < p.nacc * p.Ntile) cols *= 2;
-  p.tmem_cols = cols;
+  p.nacc = kMaxAcc;
+  p.acc_pitch = p.nacc * p.Ntile + 4;
   const size_t smem_bytes = 1024 + (size_t)nst * stage + tail + 128;
 
   // ---- tensor maps

@@ -1,4 +1,4 @@
-// HBM-bound elementwise / reduction kernels of the hot path (sm_100a): weight (un)packing, the
+// HBM-bound elementwise / reduction kernels of the hot path (sm_90a): weight (un)packing, the
 // GroupNorm finalize / apply split, GroupNorm+ReLU+Dropout backward (two-pass: per-(n,c) sums,
 // then dy = g*P + y*Q + R), bias column sums, 2x max-pooling, head sigmoid/softmax.
 //
@@ -873,7 +873,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
 // Fused GroupNorm+ReLU+Dropout backward for the SMALL pyramid levels: gn_bwd_reduce -> grid barrier -> gn_bwd_apply in
 // ONE launch.  At 24^3 and below each of the two kernels is a few microseconds of launch + prologue around almost no
 // data; the tensors stay in L2 between the phases.  Requirements (checked by the host): every CTA of the grid is
-// resident at the same time (grid <= SMs x occupancy), channel groups are a power of two <= 32 (the staged
+// resident at the same time (grid <= SMs x occupancy), channel groups are a power of two <= 256 (the staged
 // reduction), fused coefficients.  `counter` is a zero-initialised word owned by this launch (one-shot barrier).
 template <typename T, int VEC>
 __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restrict__ g, long long ldg,
@@ -915,6 +915,10 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
   }
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int lane_groups = G < 32 ? G : 32;
+  if (G > 32) {     // a warp covers only part of the channels: rows it does not write stay zero
+    for (int i = threadIdx.x; i < 24 * C; i += blockDim.x) s_part[i] = 0.f;
+    __syncthreads();
+  }
 #pragma unroll
   for (int j = 0; j < VEC; ++j) {
     for (int off = 16; off >= lane_groups; off >>= 1) {
@@ -1302,7 +1306,7 @@ int ew_gn_bwd_fused_supported(const b200seg_tensor* g, const b200seg_tensor* y, 
   if (!(vec_ok(g) && vec_ok(y) && vec_ok(dy))) return 0;
   const int vec = y->dtype == B200SEG_BF16 ? 8 : 4;
   const int G = y->c / vec;
-  if (G < 1 || G > 32 || (G & (G - 1)) != 0 || y->c > 512) return 0;
+  if (G < 1 || G > 256 || (G & (G - 1)) != 0 || y->c > 512) return 0;
   const long long elems = nvox(y) * y->c * (long long)y->n;
   return elems <= (4ll << 20) ? 1 : 0;          // <= 4 Mi elements: the 24^3 x 64 level and below
 }

@@ -1,4 +1,4 @@
-// Fused segmentation losses (sm_100a): ONE reduction pass over logits + labels producing every
+// Fused segmentation losses (sm_90a): ONE reduction pass over logits + labels producing every
 // partial sum the Dice / BCE / CE / focal family needs, a scalar finalize, and ONE elementwise
 // backward pass writing d loss / d logits (closed forms: SURVEY.md App. C; reference formulas:
 // model/losses.py:43-53,141-147,160-181,252-260,273-285,301-325).
@@ -473,8 +473,7 @@ static int loss_blocks(long long nvox_, int device) {
 // blocks per sample for the (blocks, N) grids of the partial-sum kernels
 static dim3 sample_grid(long long vox, int N, int device) {
   // blocks per SM over the whole grid: every block ends in one fp64 atomic per partial sum (15 for two classes) on
-  // the SAME few addresses, so more blocks buy load parallelism and pay in serialised atomics.  Measured on B200,
-  // VNet3d 96^3 batch 2 step (profiles/r2_overlap_ab.jsonl): 8 -> 3.145 ms, 4 -> 3.137 ms, 2 -> 3.150 ms
+  // the SAME few addresses, so more blocks buy load parallelism and pay in serialised atomics (B200SEG_LOSS_BPS)
   const char* e = getenv("B200SEG_LOSS_BPS");          // read per call (host side, once per launch): in-process A/B
   const int v = e ? atoi(e) : 0;
   const int bps = v >= 1 && v <= 16 ? v : 4;

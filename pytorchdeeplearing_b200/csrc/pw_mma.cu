@@ -1,10 +1,9 @@
-// 1x1x1 convolutions at 16..64 channels on mma.sync (sm_100a, bf16): VNet3d.py:64 up-path `conv` (2C -> C after the
+// 1x1x1 convolutions at 16..64 channels on mma.sync (sm_90a, bf16): VNet3d.py:64 up-path `conv` (2C -> C after the
 // skip concat) and its data gradient.
 //
-// These layers do 32..128 MACs per byte: they are HBM streams with a small GEMM attached.  On the tcgen05/TMA path
-// (conv_tc.cu) every 128-voxel tile pays a TMA issue, an mbarrier round trip into the MMA warp, a TMEM accumulator
-// hand-over and a tcgen05.ld before a single byte is stored, and the layer runs at ~1/3 of the HBM rate.  Here the
-// GEMM stays in registers:
+// These layers do 32..128 MACs per byte: they are HBM streams with a small GEMM attached.  On the wgmma/TMA path
+// (conv_tc.cu) every 128-voxel tile pays a TMA issue, an mbarrier round trip into the MMA warpgroup and an
+// accumulator hand-over through shared memory before a single byte is stored.  Here the GEMM stays in registers:
 //   * a CTA copies 512 consecutive voxels x Cin (one contiguous run of the NDHWC tensor, or pitched rows of a
 //     concat buffer) into shared memory with 16-byte cp.async, double buffered;
 //   * each of the 8 warps multiplies four 16-voxel row groups: A fragments by ldmatrix (rows padded by 16 B: no bank
@@ -241,7 +240,7 @@ int pw_mma_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, c
   }
   const long long V = (long long)x->d * x->h * x->w;
   if (V % PW_TILE != 0) return 0;
-  if ((long long)y->d * y->h * y->w * y->n < 65536) return 0;         // small levels stay on the tcgen05 kernel
+  if ((long long)y->d * y->h * y->w * y->n < 65536) return 0;         // small levels stay on the wgmma kernel
   return 1;
 }
 

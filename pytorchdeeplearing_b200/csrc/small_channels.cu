@@ -1,4 +1,4 @@
-// CUDA-core kernels for the layers that are NOT dense MMAs (sm_100a): the stem (Cin = image channels, 1..4)
+// CUDA-core kernels for the layers that are NOT dense MMAs (sm_90a): the stem (Cin = image channels, 1..4)
 // and the head (Cout = number of classes, 1..8).  These layers move full-resolution tensors with a
 // handful of FLOPs per byte, so they are written as HBM-streaming stencil / pointwise kernels:
 // one thread per voxel, 128-bit channel-vector stores/loads, weights in shared memory.

@@ -1,4 +1,4 @@
-// Device-side input staging (sm_100a): what the reference's datasets do to a batch on the host before the step,
+// Device-side input staging (sm_90a): what the reference's datasets do to a batch on the host before the step,
 // done on the GPU from the raw 8-bit images so that a step moves 1 byte per voxel over PCIe instead of 4 + 8.
 //   stage_u8_sums / stage_u8_normalize : datasetModelSegwithopencv.__getitem__ (model/dataset.py:138-142):
 //       image = (image - image.mean()) / image.std()   on the resized 8-bit image (numpy: float64, population std)

@@ -1,4 +1,4 @@
-// Single-image-channel stem (Cin == 1) on CUDA cores (sm_100a): VNet3d.py:28-29 in_tr.conv1 (3x3x3) /
+// Single-image-channel stem (Cin == 1) on CUDA cores (sm_90a): VNet3d.py:28-29 in_tr.conv1 (3x3x3) /
 // in_tr.conv2 (1x1x1), Unet3d.py:67 / Unet2d.py:67 enc1conv1.  These two layers carry 27 (or 1) MACs per output
 // element -- no MMA shape fits -- but they touch full-resolution tensors, so they must run at streaming speed:
 //

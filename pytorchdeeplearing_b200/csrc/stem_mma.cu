@@ -1,7 +1,7 @@
-// bf16 stem (Cin == 1) on the warp-level tensor-core path (mma.sync m16n8k16, sm_100a).
+// bf16 stem (Cin == 1) on the warp-level tensor-core path (mma.sync m16n8k16, sm_90a).
 //
 // The stem has one input channel: as a GEMM its K dimension is just the taps (27 -> padded to 32), far too thin
-// for a tcgen05 tile, and on CUDA cores the 27-tap stencil is bound by shared-memory weight broadcasts (forward)
+// for a wgmma tile, and on CUDA cores the 27-tap stencil is bound by shared-memory weight broadcasts (forward)
 // or by load latency with 72 live accumulators (weight gradient).  Both directions are re-stated here as tiny
 // im2col GEMMs whose operand fragments are gathered straight from a halo tile of the image in shared memory:
 //

@@ -1,9 +1,10 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and the lazily-resolved cuTensorMapEncodeTiled entry point,
-// shared by the tensor-core kernels (conv_tc.cu, wgrad_tc.cu).  sm_100a only.
+// wgmma / TMA / mbarrier PTX wrappers and the lazily-resolved cuTensorMapEncodeTiled entry point,
+// shared by the tensor-core kernels (conv_tc.cu, wgrad_tc.cu, conv_halo.cu, conv_halo_ws.cu).  sm_90a.
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b200seg {
 
@@ -46,8 +47,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -79,68 +78,71 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// wgmma: a warpgroup (four warps, the first a multiple of four) computes 64 rows into fp32 registers; thread t (warp
+// w = t/32, lane l) holds in d[i] row 16w + l/4 + 8((i/2)&1), column 8(i/4) + 2(l&3) + (i&1).  wgmma_fence reconverges
+// the warp first (the instructions are .aligned; barrier waits can leave it diverged).
+__device__ __forceinline__ void wgmma_fence() {
+  __syncwarp();
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread i of the warp gets TMEM lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void frag_zero(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
+}
+// accumulator fragment (64 rows starting at row0) <-> a row-major fp32 tile in shared memory, `pitch` floats per row
+template <int R>
+__device__ __forceinline__ void frag_store(float* s, int pitch, int row0, const float (&d)[R], int wt) {
+  const int r = row0 + 16 * (wt >> 5) + ((wt & 31) >> 2), c = 2 * (wt & 3);
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(s + r * pitch + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(s + (r + 8) * pitch + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+template <int R>
+__device__ __forceinline__ void frag_load(const float* s, int pitch, int row0, float (&d)[R], int wt) {
+  const int r = row0 + 16 * (wt >> 5) + ((wt & 31) >> 2), c = 2 * (wt & 3);
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    const float2 a = *reinterpret_cast<const float2*>(s + r * pitch + 8 * j + c);
+    const float2 b = *reinterpret_cast<const float2*>(s + (r + 8) * pitch + 8 * j + c);
+    d[4 * j] = a.x; d[4 * j + 1] = a.y; d[4 * j + 2] = b.x; d[4 * j + 3] = b.y;
+  }
+}
+// 16 consecutive fp32 of one accumulator row in shared memory (16-byte aligned)
+__device__ __forceinline__ void acc_ld16(const float* s, float* v) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 f = reinterpret_cast<const float4*>(s)[j];
+    v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
+  }
 }
 
-// 32 lanes x 16 consecutive fp32 columns <- zero (accumulators that are only ever accumulated into)
-__device__ __forceinline__ void tmem_st16_zero(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-      ::"r"(taddr), "r"(z)
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
+// Shared-memory matrix descriptors (layout type in bits 62-63: 1 = 128-byte, 2 = 64-byte, 3 = 32-byte swizzle).
 // K-major, swizzled operand tile (rows of `swizzle_bytes`, 8-row atoms): SBO = 8 * swizzle_bytes
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, uint32_t swizzle_bytes) {
-  const uint64_t layout = swizzle_bytes == 128 ? 2ull : (swizzle_bytes == 64 ? 4ull : 6ull);
+  const uint64_t layout = swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : 3ull);
   const uint64_t sbo = (uint64_t)(8u * swizzle_bytes) >> 4;
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (sbo << 32) | (1ull << 46) | (layout << 61);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
 }
 
 
 // MN-major, swizzled operand tile: rows (K index) of `swizzle_bytes` holding swizzle_bytes/2 bf16 MN-elements,
 // 8-row atoms (SBO = 8 * swizzle_bytes); the next group of MN-elements starts `lbo_bytes` further on.
 __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t swizzle_bytes, uint32_t lbo_bytes) {
-  const uint64_t layout = swizzle_bytes == 128 ? 2ull : (swizzle_bytes == 64 ? 4ull : 6ull);
+  const uint64_t layout = swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : 3ull);
   const uint64_t sbo = (uint64_t)(8u * swizzle_bytes) >> 4;
   const uint64_t lbo = (uint64_t)lbo_bytes >> 4;
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (lbo << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (lbo << 16) | (sbo << 32) | (layout << 62);
 }
 
 }  // namespace b200seg

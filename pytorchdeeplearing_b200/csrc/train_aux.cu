@@ -1,4 +1,4 @@
-// Kernels around the conv path of one training / inference step (sm_100a):
+// Kernels around the conv path of one training / inference step (sm_90a):
 //   adam_tick + adam_step   : fused Adam / AdamW over FLAT fp32 parameter / gradient / moment buffers
 //                             (optim.AdamW(lr) model/modelVNet.py:548; optim.Adam model/modelUnet.py:849) -- SURVEY 8f-1
 //   dropout_masks_kernel    : ALL nn.Dropout3d/2d(p) channel masks of one forward in one launch, reproducing the

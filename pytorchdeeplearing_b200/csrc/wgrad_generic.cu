@@ -1,4 +1,4 @@
-// Generic weight-gradient kernel on CUDA cores (fp32 FFMA) for sm_100a.
+// Generic weight-gradient kernel on CUDA cores (fp32 FFMA) for sm_90a.
 //
 //   dwp[t][ka][kb] += sum_{n,o} a[n, o*s + t - p, ka] * b[n, o, kb]
 //

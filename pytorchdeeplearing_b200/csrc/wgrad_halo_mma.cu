@@ -1,4 +1,4 @@
-// Weight gradient of the full-resolution 3x3x3 layers (16/32 channels) from halo tiles, on mma.sync (sm_100a, bf16).
+// Weight gradient of the full-resolution 3x3x3 layers (16/32 channels) from halo tiles, on mma.sync (sm_90a, bf16).
 //
 //   dW[tap][ci][co] += sum_v x[v + tap][ci] * dy[v][co]
 //

@@ -1,20 +1,20 @@
-// tcgen05 + TMA weight-gradient kernel for sm_100a (bf16 operands, fp32 accumulation in TMEM).
+// wgmma + TMA weight-gradient kernel for sm_90a (bf16 operands, fp32 accumulation in registers).
 //
 //   dwp[t][ka][kb] += sum_{n,o} a[n, o + t - p, ka] * b[n, o, kb]        (stride-1 kinds: 3x3x3 / 3x3 / 1x1)
 //
 // GEMM view: M = flattened (tap, ka) rows, N = kb, K = output voxels.  Both operands sit in shared
 // memory exactly as TMA delivers NDHWC boxes -- [voxel rows][channels] -- which is the MN-major
-// canonical UMMA layout (rows = K index, 32/64/128-byte swizzled rows of MN elements), so no
+// canonical wgmma layout (rows = K index, 32/64/128-byte swizzled rows of MN elements), so no
 // transposition is ever materialised:
 //   A stage : 128/CA sub-tiles, each the activation box of one (tap, 16/32/64-channel block) shifted
 //             by the tap offset (TMA zero fill = conv padding); consecutive sub-tiles are consecutive
 //             MN atoms (descriptor LBO = sub-tile bytes), i.e. several taps are STACKED along M so
-//             that 16- and 32-channel layers still fill the M = 128 instruction.
-//   B stage : the dy box of the same 128 voxels, kb channels in 64-channel sub-tiles.
-//   MMA     : 8 x tcgen05.mma (M128 x N=kb x K16 voxels) per stage, a_major = b_major = MN.
-// A CTA owns a contiguous chunk of voxel tiles and up to 512/kb accumulator blocks (128 rows each)
-// resident in TMEM for its whole lifetime; the epilogue adds them into dwp with vectorised fp32 atomics
-// (split-K over the grid).  Warp roles as in conv_tc.cu.
+//             that 16- and 32-channel layers still fill the 128-row accumulator block.
+//   B stage : the dy box of the same 128 voxels, the CTA's NC kb channels in 64-channel sub-tiles.
+//   MMA     : 2 x 8 wgmma (two M64 halves x N=NC x K16 voxels) per stage, both operands MN-major.
+// A CTA owns one accumulator block (128 rows x NC columns, in the registers of its MMA warpgroup) and a contiguous
+// chunk of voxel tiles; at the end the warpgroup adds the block into dwp with fp32 atomics (split-K over the grid).
+// Warp roles (256 threads): warp 0 TMA producer, warps 1-3 idle, warps 4-7 MMA warpgroup + epilogue.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -28,29 +28,30 @@ struct WgArgs {
   int kd, kh, kw, pd, ph, pw, sd, sh, sw;
   int bw, bh, bd, tw, th, td, ntiles;
   int CA, CB;                // channels per A / B sub-tile (<= 64)
-  int mblocks_total, mb_per_cta;
-  int nstages, tmem_cols;
+  int mblocks_total;
+  int nstages;
 };
 
 constexpr int kWgMaxStages = 6;
+constexpr int kWgThreads = 256;
 
-__global__ void __launch_bounds__(192, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                          const __grid_constant__ CUtensorMap tmB, const WgArgs p) {
+// grid: x = split-K over the voxel tiles, y = accumulator block (128 rows of (tap, ka)), z = group of NC columns
+template <int NC>
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                 const __grid_constant__ CUtensorMap tmB, const WgArgs p) {
   PDL_TRIGGER();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t A_SUB = 128u * (uint32_t)p.CA * 2u;          // bytes of one A sub-tile
   const uint32_t A_BYTES = 128u * 128u * 2u;                  // 128/CA sub-tiles
   const uint32_t B_SUB = 128u * (uint32_t)p.CB * 2u;
-  const uint32_t nbsub = (uint32_t)(p.Kb / p.CB);
+  const uint32_t nbsub = (uint32_t)(NC / p.CB);
   const uint32_t B_BYTES = B_SUB * nbsub;
   const uint32_t STAGE = A_BYTES + B_BYTES;
   uint8_t* tail = smem + (size_t)p.nstages * STAGE;
   uint64_t* full = reinterpret_cast<uint64_t*>(tail);
   uint64_t* empty = full + kWgMaxStages;
-  uint64_t* tfull = empty + kWgMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 2);
-  int4* s_sub = reinterpret_cast<int4*>(tmem_slot + 4);       // [mb_per_cta][128/CA] : channel, dw, dh, dd of a sub-tile
+  int4* s_sub = reinterpret_cast<int4*>(empty + kWgMaxStages);   // [128/CA] : channel, dw, dh, dd of a sub-tile
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -58,27 +59,24 @@ __global__ void __launch_bounds__(192, 1) wgrad_tc_kernel(const __grid_constant_
   const int tiles_per_cta = (p.ntiles + gridDim.x - 1) / gridDim.x;
   const int tile_begin = blockIdx.x * tiles_per_cta;
   const int tile_end = min(p.ntiles, tile_begin + tiles_per_cta);
-  const int mb0 = blockIdx.y * p.mb_per_cta;
-  const int nmb = min(p.mb_per_cta, p.mblocks_total - mb0);
+  const int mb = blockIdx.y;
+  const int col0 = blockIdx.z * NC;
   const int nasub = 128 / p.CA;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nstages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 4);      // one arrive per MMA warp
     }
-    mbar_init(&tfull[0], 1);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  // tap decode of every A sub-tile this CTA will ever load (keeps integer division out of the producer loop)
-  for (int i = threadIdx.x; i < nmb * nasub; i += blockDim.x) {
-    const int mb = i / nasub, j = i - mb * nasub;
-    const int R = (mb0 + mb) * 128 + j * p.CA;
+  // tap decode of every A sub-tile of this CTA's block (keeps integer division out of the producer loop)
+  for (int j = threadIdx.x; j < nasub; j += blockDim.x) {
+    const int R = mb * 128 + j * p.CA;
     int4 e = make_int4(-1, 0, 0, 0);
     if (R < p.Rtot) {
       const int tap = R / p.Ka;
@@ -87,107 +85,87 @@ __global__ void __launch_bounds__(192, 1) wgrad_tc_kernel(const __grid_constant_
       e.z = (tap / p.kw) % p.kh - p.ph;
       e.w = tap / (p.kw * p.kh) - p.pd;
     }
-    s_sub[i] = e;
+    s_sub[j] = e;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   PDL_WAIT();               // everything above is on-chip set-up: it runs under the tail of the previous kernel
-  const bool has_work = tile_begin < tile_end && nmb > 0;
+  if (tile_begin >= tile_end) return;
 
   if (warp == 0) {
     // ===================================================== TMA producer
-    if (has_work && elect_one()) {
+    if (elect_one()) {
+      // the last M block may be partial: skip (and do not expect) the sub-tiles that do not exist
+      int valid = 0;
+      for (int j = 0; j < nasub; ++j) valid += s_sub[j].x >= 0 ? 1 : 0;
       uint32_t it = 0;
-      for (int tile = tile_begin; tile < tile_end; ++tile) {
+      for (int tile = tile_begin; tile < tile_end; ++tile, ++it) {
         int t = tile;
         const int iw = t % p.tw; t /= p.tw;
         const int ih = t % p.th; t /= p.th;
         const int id = t % p.td;
         const int n = t / p.td;
         const int w0 = iw * p.bw, h0 = ih * p.bh, d0 = id * p.bd;
-        for (int mb = 0; mb < nmb; ++mb, ++it) {
-          const uint32_t s = it % p.nstages;
-          const uint32_t ph = (it / p.nstages) & 1u;
-          mbar_wait(&empty[s], ph ^ 1u);
-          uint8_t* sa = smem + (size_t)s * STAGE;
-          // the last M block may be partial: skip (and do not expect) the sub-tiles that do not exist
-          int valid = 0;
-          for (int j = 0; j < nasub; ++j) valid += s_sub[mb * nasub + j].x >= 0 ? 1 : 0;
-          mbar_expect_tx(&full[s], (uint32_t)valid * A_SUB + B_BYTES);
-          for (int j = 0; j < valid; ++j) {
-            const int4 e = s_sub[mb * nasub + j];
-            tma_load_5d(&tmA, sa + (size_t)j * A_SUB, &full[s], e.x, w0 * p.sw + e.y, h0 * p.sh + e.z, d0 * p.sd + e.w, n);
-          }
-          for (uint32_t j = 0; j < nbsub; ++j)
-            tma_load_5d(&tmB, sa + A_BYTES + (size_t)j * B_SUB, &full[s], (int)j * p.CB, w0, h0, d0, n);
+        const uint32_t s = it % p.nstages;
+        const uint32_t ph = (it / p.nstages) & 1u;
+        mbar_wait(&empty[s], ph ^ 1u);
+        uint8_t* sa = smem + (size_t)s * STAGE;
+        mbar_expect_tx(&full[s], (uint32_t)valid * A_SUB + B_BYTES);
+        for (int j = 0; j < valid; ++j) {
+          const int4 e = s_sub[j];
+          tma_load_5d(&tmA, sa + (size_t)j * A_SUB, &full[s], e.x, w0 * p.sw + e.y, h0 * p.sh + e.z, d0 * p.sd + e.w, n);
         }
+        for (uint32_t j = 0; j < nbsub; ++j)
+          tma_load_5d(&tmB, sa + A_BYTES + (size_t)j * B_SUB, &full[s], col0 + (int)j * p.CB, w0, h0, d0, n);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (has_work) {
-      // c_format f32 | a,b bf16 | a_major = b_major = MN | N | M = 128
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                             ((uint32_t)(p.Kb >> 3) << 17) | ((128u >> 4) << 24);
-      const uint32_t swa = (uint32_t)p.CA * 2u, swb = (uint32_t)p.CB * 2u;
-      uint32_t it = 0;
-      for (int tile = tile_begin; tile < tile_end; ++tile) {
-        for (int mb = 0; mb < nmb; ++mb, ++it) {
-          const uint32_t s = it % p.nstages;
-          const uint32_t ph = (it / p.nstages) & 1u;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
-            const uint64_t adesc = make_mnmajor_desc(sa, swa, A_SUB);
-            const uint64_t bdesc = make_mnmajor_desc(sa + A_BYTES, swb, B_SUB);
-            const uint32_t tacc = tmem_base + (uint32_t)(mb * p.Kb);
+  } else if (warp >= 4) {
+    // ===================================================== MMA warpgroup, then the dW epilogue
+    const int wt = threadIdx.x - 128;
+    const uint32_t swa = (uint32_t)p.CA * 2u, swb = (uint32_t)p.CB * 2u;
+    float d0[NC / 2], d1[NC / 2];
+    frag_zero(d0);
+    frag_zero(d1);
+    uint32_t it = 0;
+    for (int tile = tile_begin; tile < tile_end; ++tile, ++it) {
+      const uint32_t s = it % p.nstages;
+      const uint32_t ph = (it / p.nstages) & 1u;
+      mbar_wait(&full[s], ph);
+      const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
+      const uint64_t adesc = make_mnmajor_desc(sa, swa, A_SUB);
+      const uint64_t bdesc = make_mnmajor_desc(sa + A_BYTES, swb, B_SUB);
+      wgmma_fence_regs(d0);
+      wgmma_fence_regs(d1);
+      wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              // 16 voxel rows per K step: advance the start address by 16 rows of the operand's row pitch
-              const uint64_t ka = (uint64_t)((16u * swa * (uint32_t)k) >> 4);
-              const uint64_t kb = (uint64_t)((16u * swb * (uint32_t)k) >> 4);
-              umma_bf16(tacc, adesc + ka, bdesc + kb, idesc, (tile != tile_begin || k != 0) ? 1u : 0u);
-            }
-            umma_commit(&empty[s]);
-            if (tile == tile_end - 1 && mb == nmb - 1) umma_commit(&tfull[0]);
-          }
-          __syncwarp();
-        }
+      for (int k = 0; k < 8; ++k) {
+        // 16 voxel rows per K step: advance the start address by 16 rows of the operand's row pitch; rows 64..127 of
+        // the block are the A sub-tiles 64 MN elements (16 KB) further on
+        const uint64_t ka = (uint64_t)((16u * swa * (uint32_t)k) >> 4);
+        const uint64_t kb = (uint64_t)((16u * swb * (uint32_t)k) >> 4);
+        Wgmma<NC, 1, 1>::mma(d0, adesc + ka, bdesc + kb);
+        Wgmma<NC, 1, 1>::mma(d1, adesc + (uint64_t)(16384u >> 4) + ka, bdesc + kb);
       }
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_fence_regs(d0);
+      wgmma_fence_regs(d1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-  } else {
-    // ===================================================== epilogue warps (2..5)
-    if (has_work) {
-      const int q = warp & 3;
-      mbar_wait(&tfull[0], 0);
-      tc_fence_after();
-      for (int mb = 0; mb < nmb; ++mb) {
-        const int R = (mb0 + mb) * 128 + q * 32 + lane;
-        const bool valid = R < p.Rtot;
-        const uint32_t tacc = tmem_base + (uint32_t)(mb * p.Kb) + ((uint32_t)(q * 32) << 16);
-        for (int c0 = 0; c0 < p.Kb; c0 += 16) {
-          float v[16];
-          tmem_ld16(tacc + (uint32_t)c0, v);
-          if (valid) {
-            float* dst = p.dwp + (size_t)R * p.Kb + c0;
+    // fragment element i of half h: row 64h + 16w + l/4 + 8*((i/2)&1), column 8*(i/4) + 2*(l&3) + (i&1)
+    const int r0 = mb * 128 + 16 * (wt >> 5) + ((wt & 31) >> 2);
+    const int c = col0 + 2 * (wt & 3);
 #pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              atomicAdd(reinterpret_cast<float4*>(dst + j), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
-          }
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < NC / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int R = r0 + 64 * h + 8 * e;
+          const float x0 = h ? d1[4 * j + 2 * e] : d0[4 * j + 2 * e];
+          const float x1 = h ? d1[4 * j + 2 * e + 1] : d0[4 * j + 2 * e + 1];
+          if (R < p.Rtot) atomicAdd(reinterpret_cast<float2*>(p.dwp + (size_t)R * p.Kb + c + 8 * j), make_float2(x0, x1));
         }
-      }
-      tc_fence_before();
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -203,7 +181,10 @@ static int sub_channels(int c) {
 
 int wgrad_tc_init(int device, int maxsm) {
   (void)device;
-  B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
   return B200SEG_OK;
 }
 
@@ -255,57 +236,13 @@ int wgrad_tc(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* 
   p.CA = sub_channels(p.Ka);
   p.CB = sub_channels(p.Kb);
   p.mblocks_total = (p.Rtot + 127) / 128;
-  // Decomposition: grid.y = groups of accumulator blocks (128 rows of (tap, ka) each), grid.x = split-K over the
-  // voxel tiles.  Every K split adds its partial dW with fp32 atomics, i.e. grid.x * |dW| bytes of L2 atomic traffic:
-  // at the small pyramid levels (few voxel tiles, large dW) that flush, not the K loop, is the run time.  The B tile
-  // is re-loaded per accumulator block anyway, so fewer blocks per CTA (more groups, fewer K splits) costs nothing
-  // in the loop.  Pick the block count per CTA that minimises  stages * t_stage + flush / rate.
-  const int sms_ = num_sms(device);
-  const int max_mb = (512 / p.Kb) < p.mblocks_total ? (512 / p.Kb) : p.mblocks_total;
-  {
-    const double stage_bytes = 128.0 * 128.0 * 2.0 + 128.0 * p.Kb * 2.0;
-    const double stage_rows = 128.0 * (128 / p.CA) + 128.0 * (p.Kb / p.CB);             // TMA rows per stage
-    double t_stage = stage_bytes / 88e3;                                                // us: ~88 GB/s ingest per SM
-    if (t_stage < stage_rows * 1.06e-3) t_stage = stage_rows * 1.06e-3;                 // ~1 row/ns for short rows
-    const double dw_bytes = (double)p.Rtot * p.Kb * 4.0;
-    const double last_w = (double)(p.Rtot - 128 * (p.mblocks_total - 1)) / 128.0;       // the last block may be partial
-    auto estimate = [&](int mb) {
-      const int gy_ = (p.mblocks_total + mb - 1) / mb;
-      int gx_ = sms_ / gy_;
-      if (gx_ < 1) gx_ = 1;
-      if (gx_ > p.ntiles) gx_ = p.ntiles;
-      const int mbc = (p.mblocks_total + gy_ - 1) / gy_;
-      // heaviest row group (the last block of the last group may be partial)
-      const double heavy = gy_ == 1 ? (double)(mbc - 1) + last_w : (double)mbc;
-      const double stages = (double)((p.ntiles + gx_ - 1) / gx_) * heavy;
-      const double waves = gy_ > sms_ ? (double)((gy_ + sms_ - 1) / sms_) : 1.0;
-      return waves * stages * t_stage + gx_ * dw_bytes / 1.5e6;                          // us: ~1.5 TB/s of atomics
-    };
-    // default: as many accumulator blocks per CTA as TMEM holds (fewest CTAs touching a tile); switch only for a
-    // clear predicted gain (the model is calibrated on the VNet3d layer shapes, tools/microbench_ops.py)
-    int best_mb = max_mb;
-    double best = estimate(max_mb) * 0.85;
-    for (int mb = 1; mb < max_mb; ++mb) {
-      const double t = estimate(mb);
-      if (t < best - 1e-9) {
-        best = t;
-        best_mb = mb;
-      }
-    }
-    static const int forced = [] {
-      const char* e = getenv("B200SEG_WGRAD_MB");
-      return e ? atoi(e) : 0;
-    }();
-    p.mb_per_cta = forced > 0 ? (forced < max_mb ? forced : max_mb) : best_mb;
-  }
-  const int gy = (p.mblocks_total + p.mb_per_cta - 1) / p.mb_per_cta;
-  // balance the accumulator blocks over the row groups
-  p.mb_per_cta = (p.mblocks_total + gy - 1) / gy;
-  int cols = 32;
-  while (cols < p.mb_per_cta * p.Kb) cols *= 2;
-  p.tmem_cols = cols;
-  const uint32_t stage = 128u * 128u * 2u + 128u * (uint32_t)p.Kb * 2u;
-  const uint32_t tail = (2 * kWgMaxStages + 2) * 8 + 16 + 16 + (uint32_t)(p.mb_per_cta * (128 / p.CA)) * 16;
+  // Decomposition: grid.y = accumulator blocks (128 rows of (tap, ka) each), grid.z = column groups of NC <= 128 kb
+  // channels (the block lives in 128 registers per thread of one warpgroup), grid.x = split-K over the voxel tiles
+  // for the rest of the chip.  Every K split adds its partial dW with fp32 atomics.
+  const int nc = p.Kb % 128 == 0 ? 128 : (p.Kb % 64 == 0 ? 64 : p.Kb);
+  const int gy = p.mblocks_total, gz = p.Kb / nc;
+  const uint32_t stage = 128u * 128u * 2u + 128u * (uint32_t)nc * 2u;
+  const uint32_t tail = 2 * kWgMaxStages * 8 + (uint32_t)(128 / p.CA) * 16;
   const int maxsm = tc_max_smem(device);
   int nst = (int)((maxsm - 1024 - (int)tail - 256) / (int)stage);
   if (nst > kWgMaxStages) nst = kWgMaxStages;
@@ -317,11 +254,14 @@ int wgrad_tc(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* 
   if (rc != B200SEG_OK) return rc;
   rc = encode_box_map(&tmB, b, p.CB, p.bw, p.bh, p.bd);
   if (rc != B200SEG_OK) return rc;
-  int gx = num_sms(device) / gy;
+  int gx = num_sms(device) / (gy * gz);
   if (gx < 1) gx = 1;
   if (gx > p.ntiles) gx = p.ntiles;
-  dim3 grid(gx, gy);
-  launch_k(wgrad_tc_kernel, grid, 192, smem_bytes, st, tmA, tmB, p);
+  dim3 grid(gx, gy, gz);
+  if (nc == 128) launch_k(wgrad_tc_kernel<128>, grid, kWgThreads, smem_bytes, st, tmA, tmB, p);
+  else if (nc == 64) launch_k(wgrad_tc_kernel<64>, grid, kWgThreads, smem_bytes, st, tmA, tmB, p);
+  else if (nc == 32) launch_k(wgrad_tc_kernel<32>, grid, kWgThreads, smem_bytes, st, tmA, tmB, p);
+  else launch_k(wgrad_tc_kernel<16>, grid, kWgThreads, smem_bytes, st, tmA, tmB, p);
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }

@@ -3,7 +3,7 @@
 The engine turns one forward/backward of ``VNet3d`` / ``UNet3d`` / ``UNet2d`` into a sequence
 of calls on a *backend* whose methods map 1:1 onto the ``extern "C"`` entry points of
 ``include/b200seg.h`` (``_abi.CudaBackend``).  It owns no arithmetic: every FLOP and every
-byte moved happens inside a backend op (= one hand-written sm_100a kernel launch).
+byte moved happens inside a backend op (= one hand-written sm_90a kernel launch).
 
 Data layout (DESIGN.md section 3): activations are channels-last ``(N, D, H, W, C)`` views
 (2-D nets use ``D == 1``) with a channel pitch ``ld >= C`` so that producers write straight
@@ -73,11 +73,8 @@ OV_ALL = OV_PACK | OV_UNPACK | OV_TAIL | OV_ZERO
 
 
 def overlap_mask(arch: str = "vnet", dims: int = 3) -> int:
-    """``B200SEG_OVERLAP`` if set, else the measured default (one B200, A/B of CUDA-graph replays in one process,
-    ``profiles/r2_overlap_ab.jsonl``): all four options together gain 0.9 % on VNet3d 96^3 batch 2 (3.166 -> 3.137 ms
-    with the loss grid below) and 2.1 % on UNet2d 512^2 batch 8 (3.855 -> 3.769 ms) -- no single option gains on its
-    own -- and LOSE 1.9 % on UNet3d 128^3 batch 1 (3.732 -> 3.803 ms), so the 3-D UNet keeps the plain schedule.
-    Data-parallel runs keep it too: the options were validated on one GPU only."""
+    """``B200SEG_OVERLAP`` if set, else the default: all four options together for VNet3d / VNet2d / UNet2d on one GPU,
+    the plain schedule for the 3-D UNet and for data-parallel runs (``tools/overlap_ab.py`` is the A/B harness)."""
     e = os.environ.get("B200SEG_OVERLAP")
     if e is not None:
         try:

@@ -23,9 +23,8 @@ everything from the deepest encoder block to the head (96 % of the bytes; comple
 done) starts its all-reduce right there and overlaps the rest of the backward, the remainder follows at the end
 (eager mode and the one-graph mode).  By default the collectives stay BETWEEN the graphs of a captured step (forward +
 loss sums | all-reduce | backward | all-reduce | optimizer).  ``B200SEG_NCCL_IN_GRAPH=1`` captures the NCCL kernels
-INSIDE one graph (thread-local capture mode, so the NCCL watchdog thread cannot invalidate the capture): measured on
-2 x B200 it replays correctly and is no faster (3.44 vs 3.43 ms per step), but tearing the process group down while
-such a graph is alive hangs on this stack (torch 2.11 / NCCL 2.28), so it is opt-in.
+INSIDE one graph (thread-local capture mode, so the NCCL watchdog thread cannot invalidate the capture); tearing the
+process group down while such a graph is alive can hang (torch 2.11 / NCCL 2.28), so it is opt-in.
 """
 from __future__ import annotations
 
@@ -186,9 +185,8 @@ class GraphedStep:
     def _capture(self):
         torch.cuda.synchronize()
         # B200SEG_HIPRI=1 captures the chain forward -> loss -> data gradients on a high-priority stream (the weight
-        # gradients run beside it on the engine's default-priority side stream).  Measured on B200: SLOWER (3.56 vs
-        # 3.28 ms per step) -- the persistent weight-gradient kernels are then starved to the end of the step instead of
-        # filling the gaps of the chain -- so it is off by default.
+        # gradients run beside it on the engine's default-priority side stream).  The persistent weight-gradient kernels
+        # are then starved to the end of the step instead of filling the gaps of the chain, so it is off by default.
         hp = None
         if os.environ.get("B200SEG_HIPRI", "0") == "1":
             hp = torch.cuda.Stream(device=self.x.device, priority=-1)

@@ -21,7 +21,7 @@ _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d",
 
 
 def install() -> int:
-    """Rebind the reference's names to the B200 implementations. Returns the number of bindings changed."""
+    """Rebind the reference's names to the drop-in implementations. Returns the number of bindings changed."""
     from . import networks as nets, losses, metric
     table = {n: getattr(nets, n) for n in _NET_NAMES}
     table.update({n: getattr(losses, n) for n in _LOSS_NAMES})

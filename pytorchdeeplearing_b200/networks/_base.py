@@ -1,5 +1,5 @@
 """Shared plumbing of the drop-in networks: one ``autograd.Function`` per forward that hands
-the whole net to the layer program (``engine.Engine``), i.e. to the sm_100a kernels."""
+the whole net to the layer program (``engine.Engine``), i.e. to the sm_90a kernels."""
 from __future__ import annotations
 
 import os
@@ -192,4 +192,4 @@ class _Holder(nn.Module):
     """Parameter container with the reference's attribute names; never called directly."""
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("sub-blocks of the B200 drop-in are parameter holders; call the network itself")
+        raise RuntimeError("sub-blocks of the drop-in are parameter holders; call the network itself")

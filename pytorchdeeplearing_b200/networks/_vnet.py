@@ -1,6 +1,6 @@
 """Shared builder of the drop-in VNet3d / VNet2d (reference networks/VNet3d.py:102-158 and its 2-D twin
 networks/VNet2d.py:102-160): same constructor signature, same ``state_dict`` (128 tensors, SURVEY.md App. A),
-forward/backward on sm_100a kernels.  The 2-D net runs through the same layer program with a unit depth."""
+forward/backward on sm_90a kernels.  The 2-D net runs through the same layer program with a unit depth."""
 import torch.nn as nn
 
 from ._base import SegNetBase, _Holder

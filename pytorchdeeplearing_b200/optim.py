@@ -1,5 +1,5 @@
 """Fused optimizer step of the training loop (SURVEY.md 8f-1): ``optim.AdamW(self.model.parameters(), lr=lr)``
-(reference model/modelVNet.py:548; ``optim.Adam`` at model/modelUnet.py:849) as ONE sm_100a kernel launch over flat
+(reference model/modelVNet.py:548; ``optim.Adam`` at model/modelUnet.py:849) as ONE sm_90a kernel launch over flat
 fp32 parameter / gradient / moment buffers (``b200seg_adam_step``) instead of ~6 foreach launches over 128 tensors.
 
     opt = FusedAdamW(model.parameters(), lr=1e-3)        # same constructor arguments as torch.optim.AdamW

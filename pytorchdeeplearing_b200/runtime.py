@@ -1,6 +1,6 @@
 """Runtime switches of the drop-in: precision mode, backend lookup, data-parallel state.
 
-There is exactly one product backend: the sm_100a CUDA library behind the C ABI of
+There is exactly one product backend: the sm_90a CUDA library behind the C ABI of
 ``include/b200seg.h`` (``_abi.CudaBackend``).  There is NO CPU / eager / library fallback:
 if the library is missing or the tensors are not on a CUDA device the call raises.
 ``_set_backend_for_testing`` exists so the CPU test-suite can drive the host-side layer
@@ -58,7 +58,7 @@ def get_backend(t: torch.Tensor):
         return _TEST_BACKEND
     if not t.is_cuda:
         raise RuntimeError(
-            "pytorchdeeplearing_b200 runs only on a CUDA (sm_100a) device: got a tensor on "
+            "pytorchdeeplearing_b200 runs only on a CUDA (sm_90a) device: got a tensor on "
             f"'{t.device}'. There is no CPU fallback -- move the model and inputs to cuda.")
     return cuda_backend()
 

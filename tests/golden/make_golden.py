@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by RUNNING THE UNMODIFIED REFERENCE in the build container.
 
-Usage (build container only; /root/reference does not exist on the GPU box):
+Usage (build container only; $PYTORCHDEEPLEARING_REFERENCE does not exist on the GPU box):
     python tests/golden/make_golden.py
 
-The reference modules are imported from /root/reference (read-only) with
+The reference modules are imported from $PYTORCHDEEPLEARING_REFERENCE (read-only) with
   * the non-invasive ``VNet3d`` constructor shim for the ``networks/VNet3d.py:127`` typo
     (``self.feature`` vs ``self.features``), and
   * a stub ``model`` package so that ``model/losses.py`` can be imported without the absent
@@ -25,7 +25,7 @@ sys.dont_write_bytecode = True
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.environ.get("PYTORCHDEEPLEARING_REFERENCE", "reference")
 sys.path.insert(0, REF)
 
 import oracle  # noqa: E402

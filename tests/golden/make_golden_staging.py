@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """tests/golden/staging.npz: what the reference's OWN 2-D dataset class returns for a few 8-bit PNG files.
 
-Build container only (needs /root/reference and cv2):    python tests/golden/make_golden_staging.py
+Build container only (needs $PYTORCHDEEPLEARING_REFERENCE and cv2):    python tests/golden/make_golden_staging.py
 
 Writes random 8-bit images / label masks as PNG into a temporary directory, reads them back through the unmodified
 ``datasetModelSegwithopencv`` (model/dataset.py:120-158; targetsize == file size, so cv2.resize is the identity) and
@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+REF = os.environ.get("PYTORCHDEEPLEARING_REFERENCE", "reference")
 
 
 def main():

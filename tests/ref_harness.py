@@ -1,18 +1,19 @@
-"""Import the UNMODIFIED reference tree (/root/reference, build container only) for drop-in tests -- TEST-ONLY.
+"""Import the UNMODIFIED reference tree (a checkout of junqiangchen/PytorchDeepLearing named by the environment variable
+PYTORCHDEEPLEARING_REFERENCE) for drop-in tests -- TEST-ONLY.
 
 The reference's ``model`` package imports four I/O-only modules that are absent here (SimpleITK, torchsummary,
 skimage, matplotlib; SURVEY.md 0.10 / App. E).  They are replaced by inert stubs in ``sys.modules``; nothing of the
-reference is modified or copied.  Tests using this harness skip when /root/reference does not exist (GPU box)."""
+reference is modified or copied.  Tests using this harness skip when no reference checkout is named."""
 import importlib
 import os
 import sys
 import types
 
-REF = "/root/reference"
+REF = os.environ.get("PYTORCHDEEPLEARING_REFERENCE", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF, "networks"))
+    return bool(REF) and os.path.isdir(os.path.join(REF, "networks"))
 
 
 def _stub(name, **attrs):

@@ -38,7 +38,7 @@ def test_library_loads_and_exports_every_declared_symbol():
     # pure host-side query, no device needed
     assert lib.b200seg_conv_tc_eligible(0, 32, 32) == 1
     assert lib.b200seg_conv_tc_eligible(0, 1, 16) == 0
-    assert lib.b200seg_conv_tc_eligible(2, 32, 64) == 1       # k2s2 down conv runs on tcgen05 too
+    assert lib.b200seg_conv_tc_eligible(2, 32, 64) == 1       # k2s2 down conv runs on the tensor-core path too
     assert lib.b200seg_conv_tc_eligible(3, 32, 48) == 0       # transposed conv needs power-of-two Cout
     assert lib.b200seg_conv_halo_eligible(0, 16, 16) == 1 and lib.b200seg_conv_halo_eligible(0, 64, 64) == 0
 

@@ -1,4 +1,4 @@
-"""Every hot-path loss class of the drop-in (SURVEY.md rows a11-a18) on the B200, through the C ABI, against
+"""Every hot-path loss class of the drop-in (SURVEY.md rows a11-a18) on the GPU, through the C ABI, against
 (1) the fixtures the REAL reference produced (tests/golden/losses.npz: value + d loss / d logits, including the
 absent-class and gamma=3 cases; reference model/losses.py:33-53,129-197,247-342) and (2) the CPU oracle on other
 shapes / class counts.  Closes the CUDA-vs-reference gap for BinaryDice / BinaryCE / BinaryFocal / MutilCE."""

@@ -1,4 +1,4 @@
-"""Per-entry-point parity of the sm_100a kernels (through the C ABI) against the test-only
+"""Per-entry-point parity of the sm_90a kernels (through the C ABI) against the test-only
 PyTorch statement of the same op (tests/emu_backend.py, CPU fp32/fp64).  `-m gpu`."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Network-level parity on the B200 (through the public nn.Module API and the C ABI):
+"""Network-level parity on the GPU (through the public nn.Module API and the C ABI):
 parity mode (fp32) must match the CPU oracle to 1e-3 relative with identical argmax masks
 (BASELINE.json north_star); perf mode (bf16) is checked against its documented error budget.
 Golden fixtures come from the real reference (tests/golden/make_golden.py)."""

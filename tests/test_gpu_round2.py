@@ -233,7 +233,7 @@ def test_unet2d_512_full_size_parity_fp32():
 
 # ------------------------------------------------------------------------------------------------ bf16 mode
 def test_bf16_vnet3d_96_vs_oracle_at_the_benchmarked_size():
-    """The benchmarked configuration (VNet3d(1,2), 2x96^3, bf16 storage, tcgen05 / mma.sync kernels) against the fp32
+    """The benchmarked configuration (VNet3d(1,2), 2x96^3, bf16 storage, wgmma / mma.sync kernels) against the fp32
     CPU oracle: the error budget of bf16 storage (SURVEY.md 0.8: ~1e-2 normwise, < 1 % argmax flips), measured here."""
     b200.set_precision("bf16")
     spec, sd, model, ofwd, _ = _build("vnet3d", 1, 2, seed=0)
@@ -266,7 +266,7 @@ def test_bf16_vnet3d_96_vs_oracle_at_the_benchmarked_size():
 ])
 @pytest.mark.parametrize("train", [False, True])
 def test_bf16_kernels_vs_cpu_emulation_of_the_same_bf16_data_flow(kind, cin, ncls, spatial, n, lossname, train):
-    """The bf16 kernel set (tcgen05 / halo / mma.sync) against the CPU emulation of the SAME data flow (bf16 storage of
+    """The bf16 kernel set (wgmma / halo / mma.sync) against the CPU emulation of the SAME data flow (bf16 storage of
     activations, gradients and packed weights, fp32 accumulation: tests/emu_backend.py), network level, eval and train
     mode.  Two bf16 evaluations that differ only in accumulation order round ~half of their 1-ulp decisions
     differently at every layer, so at network level they are as far from each other as each is from the fp32 oracle

@@ -1,4 +1,4 @@
-"""tcgen05 + TMA convolution path (bf16) against the test-only PyTorch statement of the op:
+"""wgmma + TMA convolution path (bf16) against the test-only PyTorch statement of the op:
 forward and data-gradient forms, 3x3x3 / 3x3 / 1x1, ragged volumes (box overhang), channel-pitched
 (concat-slice) inputs and outputs, fused GroupNorm statistics, fused residual addend.  `-m gpu`."""
 import pytest
@@ -60,9 +60,9 @@ def test_tc_conv_matches_emulation(be, kind, dims, n, sp, cin, cout, which):
     xbuf = (torch.randn((n,) + sp + (ci + 16,), generator=g)).to(dt)
     x = xbuf[..., 8:8 + ci]                # channel-pitched view (concat slice)
     if not be.lib.b200seg_conv_tc_eligible(kind, ci, co):
-        pytest.skip("shape not on the tcgen05 path")
+        pytest.skip("shape not on the wgmma path")
     wp_c = be.pack_weight(w.cuda(), kind, which, dt, dims)
-    assert wp_c.code == 2, "expected the tcgen05 layout"
+    assert wp_c.code == 2, "expected the wgmma layout"
     wp_e = EMU.pack_weight(w, kind, which, dt, dims)
     for with_stats, with_addend, with_bias in ((True, False, True), (False, True, False)):
         y_e = torch.zeros((n,) + sp + (co,), dtype=dt)
@@ -221,7 +221,7 @@ def _out_sp(kind, dims, sp):
 
 @pytest.mark.parametrize("kind,dims,n,sp,cin,cout", RESAMPLE_CASES)
 def test_tc_down_up_forward_dgrad_wgrad(be, kind, dims, n, sp, cin, cout):
-    """k2s2 conv / transposed conv on the tcgen05 path: forward, data gradient (the opposite form) and
+    """k2s2 conv / transposed conv on the wgmma path: forward, data gradient (the opposite form) and
     weight gradient (strided TMA gather), all against the emulation."""
     g = torch.Generator().manual_seed(11)
     dt = torch.bfloat16

@@ -5,7 +5,7 @@ kernel's index rule
     dst[t'][k][n2][n1] = src[t*st + k*sk + n2*sn2 + n1*sn1],   t' = T-1-t if flip else t      (elementwise.cu)
 
 and compared with the layout every packed-operand code promises (DESIGN.md section 3): the CUDA-core layouts against
-the CPU emulation backend's own ``pack_weight``, the tcgen05 layouts (K-major rows, 8-channel halo planes, 64-channel
+the CPU emulation backend's own ``pack_weight``, the tensor-core layouts (K-major rows, 8-channel halo planes, 64-channel
 weight-streaming groups) against direct permutations of the torch weight.  No GPU, no kernel launch: the library is
 only asked which kernel family takes a shape (pure host functions)."""
 import itertools

@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Per-kernel SASS digest of libb200seg.so: which tensor / copy paths each kernel really uses.
 
-    python tools/sass_digest.py > profiles/r2_sass_digest.txt
+    python tools/sass_digest.py > sass_digest.txt
 
-Counts the Blackwell-native mnemonics (B200_PROFILING.md): UTC*MMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st,
-UTMALDG/UTMASTG/UBLKCP = TMA, HMMA = legacy mma.sync, LDGSTS = cp.async, plus griddepcontrol (ACQBULK / PDL)."""
+Counts the Hopper mnemonics: HGMMA = wgmma, UTMALDG/UTMASTG/UBLKCP = TMA, HMMA = mma.sync, LDGSTS = cp.async."""
 import collections
 import os
 import re
@@ -13,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "pytorchdeeplearing_b200", "csrc", "libb200seg.so")
-PAT = {"UTC*MMA(tcgen05.mma)": r"\bUTC\w*MMA\b", "LDTM(tcgen05.ld)": r"\bLDTM\b", "STTM(tcgen05.st)": r"\bSTTM\b",
+PAT = {"HGMMA(wgmma)": r"\bHGMMA\b",
        "UTMALDG(TMA load)": r"\bUTMALDG\b", "UTMASTG(TMA store)": r"\bUTMASTG\b", "UBLKCP(bulk copy)": r"\bUBLKCP\b",
        "HMMA(mma.sync)": r"\bHMMA\b", "LDGSTS(cp.async)": r"\bLDGSTS\b", "FFMA": r"\bFFMA\b", "DFMA/DADD": r"\bD(FMA|ADD|MUL)\b"}
 
@@ -33,7 +32,7 @@ for line in out.splitlines():
 dem = subprocess.run(["cu++filt"] + list(counts), stdout=subprocess.PIPE, text=True).stdout.splitlines() \
     if counts else []
 names = {k: (d if d else k) for k, d in zip(counts, dem)}
-print(f"SASS digest of {os.path.relpath(LIB, ROOT)} ({len(counts)} kernels, sm_100a)")
+print(f"SASS digest of {os.path.relpath(LIB, ROOT)} ({len(counts)} kernels, sm_90a)")
 cols = list(PAT)
 print(" | ".join(["kernel"] + cols))
 tot = collections.Counter()
