@@ -16,6 +16,10 @@ import torch
 K3, K1, DOWN, UP = 0, 1, 2, 3
 F32, BF16, BF16_TC, BF16_HALO, BF16_HALO_WS = 0, 1, 2, 3, 4
 I64 = 16
+# voxels per sample a 3x3x3 layer needs before its weights are packed for the halo-staged kernels (16/32 channels)
+# and the weight-streaming halo kernel (64/128 channels); smaller layers take the TMA implicit-GEMM kernel
+HALO_MIN_VOX = 128 * 128
+HALO_WS_MIN_VOX = 1000
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libb200seg.so")
@@ -170,6 +174,7 @@ class _PackPlan:
 
 class CudaBackend:
     name = "cuda-sm90a"
+    use_tc = True      # bf16 convolutions of the shapes the library accepts always take its tensor-core kernels
 
     def __init__(self):
         if not torch.cuda.is_available():
@@ -177,12 +182,6 @@ class CudaBackend:
                                "and there is no CPU fallback")
         self.lib = load_library()
         self._inited = set()
-        # B200SEG_DISABLE_TC=1 forces every conv onto the CUDA-core implicit-GEMM kernels (debug / A-B timing)
-        self.use_tc = os.environ.get("B200SEG_DISABLE_TC", "0") != "1"
-        self.use_halo = os.environ.get("B200SEG_DISABLE_HALO", "0") != "1"
-        self.halo_min_vox = int(os.environ.get("B200SEG_HALO_MIN_VOX", str(128 * 128)))
-        self.use_halo_ws = os.environ.get("B200SEG_DISABLE_HALO_WS", "0") != "1"
-        self.halo_ws_min_vox = int(os.environ.get("B200SEG_HALO_WS_MIN_VOX", "1000"))
         self._keep_tables = []     # device descriptor tables stay referenced while launches that read them may be pending
         self.launch_count = 0      # kernels launched through the C ABI (one per successful entry-point call)
 
@@ -207,8 +206,8 @@ class CudaBackend:
         a, b = w.shape[0], w.shape[1]
         t = w.numel() // (a * b)
         od = F32 if dtype == torch.float32 else BF16
-        if (allow_tc and self.use_tc and self.use_halo_ws and dtype == torch.bfloat16 and kind == K3 and dims == 3
-                and vox is not None and vox >= self.halo_ws_min_vox):
+        if (allow_tc and dtype == torch.bfloat16 and kind == K3 and dims == 3
+                and vox is not None and vox >= HALO_WS_MIN_VOX):
             cin, cout = (b, a) if which == "fwd" else (a, b)
             nt = self.lib.b200seg_conv_halo_ws_ntile(kind, cin, cout)
             if nt > 0:
@@ -218,15 +217,15 @@ class CudaBackend:
                 else:                   # [ci/NT][T-1-t][co/8][ci%NT][co%8]
                     parts = [(i * nt * t, i * t * a * nt, (t, a // 8, nt, 8, 1, 8 * b * t, t, b * t, 1)) for i in range(g)]
                 return (g, t, cin // 8, nt, 8), BF16_HALO_WS, parts
-        if (allow_tc and self.use_tc and self.use_halo and dtype == torch.bfloat16 and kind == K3
-                and vox is not None and vox >= self.halo_min_vox):
+        if (allow_tc and dtype == torch.bfloat16 and kind == K3
+                and vox is not None and vox >= HALO_MIN_VOX):
             cin, cout = (b, a) if which == "fwd" else (a, b)
             if self.lib.b200seg_conv_halo_eligible(kind, cin, cout):
                 if which == "fwd":      # [t][ci/8][co][ci%8]
                     return (t, b // 8, a, 8), BF16_HALO, (t, b // 8, a, 8, 1, 8 * t, b * t, t, 0)
                 return (t, a // 8, b, 8), BF16_HALO, (t, a // 8, b, 8, 1, 8 * b * t, t, b * t, 1)   # [T-1-t][co/8][ci][co%8]
         tc = False
-        if allow_tc and self.use_tc and dtype == torch.bfloat16:
+        if allow_tc and dtype == torch.bfloat16:
             # (kind, Cin, Cout) of the op that will consume the packed operand
             if which == "fwd":
                 op = (kind, a, b) if kind == UP else (kind, b, a)
@@ -360,16 +359,13 @@ class CudaBackend:
         self._check(self.lib.b200seg_conv(kind, dims, C.byref(dx), wpk.t.data_ptr(), wpk.code, _p(bias), C.byref(dy),
                                           _p(stats), _ref(da), dev, st))
 
-    fused_bwd_stats = os.environ.get("B200SEG_FUSED_BWD_STATS", "1") != "0"
-
     def conv_bwdstats_ok(self, kind, dims, x, wpk, y, addend, yfwd):
         """can ``conv_bwdstats`` take this data-gradient convolution (3-D halo-staged 16/32-channel 3x3x3 layers)?"""
-        if (not self.fused_bwd_stats or wpk.code not in (BF16_HALO, BF16_HALO_WS) or x.dtype != torch.bfloat16
-                or y.dtype != torch.bfloat16):
+        if wpk.code not in (BF16_HALO, BF16_HALO_WS) or x.dtype != torch.bfloat16 or y.dtype != torch.bfloat16:
             return False
         # with 16 output channels the layer is traffic bound once it also reads the producer's raw output, so the
-        # fused form is used for 32 output channels only (B200SEG_BWDSTATS_ALL=1 takes it for 16 too)
-        if y.shape[-1] == 16 and os.environ.get("B200SEG_BWDSTATS_ALL", "0") != "1":
+        # fused form is used for 32 output channels only
+        if y.shape[-1] == 16:
             return False
         dx, dy, da, df = _desc(x), _desc(y), _desc(addend), _desc(yfwd)
         return bool(self.lib.b200seg_conv_bwdstats_supported(kind, dims, C.byref(dx), wpk.code, C.byref(dy), _ref(da),
@@ -401,8 +397,6 @@ class CudaBackend:
         self._check(self.lib.b200seg_apply(C.byref(d1), c1.data_ptr(), _ref(d2), _p(c2), _ref(dr), C.byref(do), dev, st))
 
     # fused-coefficient forms: gn = (stats, gamma, beta, scale|None, vox, groups, eps)
-    fused_gn = os.environ.get("B200SEG_FUSED_GN", "1") != "0"
-
     @staticmethod
     def _gn(gn):
         if gn is None:
@@ -429,11 +423,7 @@ class CudaBackend:
                                                      C.byref(dd), dgamma.data_ptr(), dbeta.data_ptr(), _p(dbias),
                                                      1 if sum_y_from_stats else 0, dev, st))
 
-    fused_gn_bwd = os.environ.get("B200SEG_FUSED_GN_BWD", "1") != "0"
-
     def gn_bwd_fused_ok(self, g, y, dy):
-        if not (self.fused_gn and self.fused_gn_bwd):
-            return False
         dev, _ = self._ds(y)
         dg, dyy, dd = _desc(g), _desc(y), _desc(dy)
         return bool(self.lib.b200seg_gn_bwd_fused_supported(C.byref(dg), C.byref(dyy), C.byref(dd), dev))

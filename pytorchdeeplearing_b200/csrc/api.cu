@@ -1,6 +1,5 @@
 // extern "C" surface of libb200seg.so (see include/b200seg.h for the contract).
 #include <stdarg.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -30,7 +29,6 @@ int conv_halo_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype
 int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, const float* bias, const b200seg_tensor* y,
               double* stats, const b200seg_tensor* addend, int device, cudaStream_t st,
               const b200seg_tensor* yfwd = nullptr, const b200seg_gn* gn = nullptr, double* sums = nullptr);
-int conv_halo_bwdstats_ok(int dims);
 int pw_mma_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                      const b200seg_tensor* addend);
 int pw_mma_conv(int kind, int dims, const b200seg_tensor* x, const void* w, const float* bias,
@@ -207,15 +205,11 @@ int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, i
   }
   B200_CHECK_ARG(w_dtype != B200SEG_BF16_TC && w_dtype != B200SEG_BF16_HALO && w_dtype != B200SEG_BF16_HALO_WS,
                  "b200seg_conv: B200SEG_BF16_TC weights need bf16, 16-byte aligned activations of a supported shape");
-  static const bool stem_off = [] {
-    const char* e = getenv("B200SEG_DISABLE_STEM");
-    return e && e[0] == '1';
-  }();
   const bool small_types =
       w_dtype == B200SEG_F32 ? (x->dtype == B200SEG_F32 && y->dtype == B200SEG_F32) : y->dtype == B200SEG_BF16;
-  if (!stem_off && stem_mma_conv_supported(kind, x, w_dtype, y, addend))
+  if (stem_mma_conv_supported(kind, x, w_dtype, y, addend))
     return stem_mma_conv(kind, dims, x, wpk, bias, y, stats, device, ST(stream));
-  if (!stem_off && small_types && stem_conv_supported(kind, x, y, addend))
+  if (small_types && stem_conv_supported(kind, x, y, addend))
     return stem_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
   if (small_types && smallcin_conv_supported(kind, x, y, addend))
     return smallcin_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
@@ -227,7 +221,7 @@ static int bwdstats_path(int kind, int dims, const b200seg_tensor* x, int w_dtyp
   // 1: halo3 (16/32 channels, 3-D), 2: halo-ws (64/128 channels), 0: none -- and only where b200seg_conv itself would
   // take that kernel
   if (pw_mma_supported(kind, dims, x, w_dtype, y, addend) || conv_tc_supported(kind, dims, x, w_dtype, y, addend)) return 0;
-  if (conv_halo_supported(kind, dims, x, w_dtype, y, addend)) return conv_halo_bwdstats_ok(dims) ? 1 : 0;
+  if (conv_halo_supported(kind, dims, x, w_dtype, y, addend)) return dims == 3 ? 1 : 0;
   if (conv_halows_supported(kind, dims, x, w_dtype, y, addend)) return 2;
   return 0;
 }
@@ -272,24 +266,15 @@ int b200seg_wgrad(int kind, int dims, const b200seg_tensor* a, const b200seg_ten
   B200_CHECK_ARG(dwp != nullptr, "b200seg_wgrad: null output");
   B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_wgrad: dims must be 2 or 3");
   B200_DEVICE(device);
-  static const bool tc_off = [] {
-    const char* e = getenv("B200SEG_DISABLE_TC_WGRAD");
-    const char* e2 = getenv("B200SEG_DISABLE_TC");
-    return (e && e[0] == '1') || (e2 && e2[0] == '1');
-  }();
-  if (!tc_off && wgrad_halo_mma_supported(kind, dims, a, b))
+  if (wgrad_halo_mma_supported(kind, dims, a, b))
     return wgrad_halo_mma(kind, dims, a, b, dwp, device, ST(stream));
-  if (!tc_off && wgrad_tc_supported(kind, dims, a, b)) {
+  if (wgrad_tc_supported(kind, dims, a, b)) {
     if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
     return wgrad_tc(kind, dims, a, b, dwp, device, ST(stream));
   }
-  static const bool stem_off = [] {
-    const char* e = getenv("B200SEG_DISABLE_STEM");
-    return e && e[0] == '1';
-  }();
-  if (!stem_off && stem_mma_wgrad_supported(kind, a, b))
+  if (stem_mma_wgrad_supported(kind, a, b))
     return stem_mma_wgrad(kind, dims, a, b, dwp, device, ST(stream));
-  if (!stem_off && stem_wgrad_supported(kind, a, b)) return stem_wgrad(kind, dims, a, b, dwp, device, ST(stream));
+  if (stem_wgrad_supported(kind, a, b)) return stem_wgrad(kind, dims, a, b, dwp, device, ST(stream));
   if (smallcin_wgrad_supported(kind, a, b)) return smallcin_wgrad(kind, dims, a, b, dwp, device, ST(stream));
   return wgrad_generic(kind, dims, a, b, dwp, device, ST(stream));
 }

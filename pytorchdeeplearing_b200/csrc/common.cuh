@@ -150,7 +150,7 @@ __device__ __forceinline__ double warp_sum(double v) {
 // the next kernel of the chain is launched and its CTAs are scheduled while the last wave of this one is still
 // running, so the launch latency (~2-3 us per boundary inside a CUDA graph) leaves the critical path.  Because the
 // wait is the first instruction, every kernel still sees the complete output of ALL its predecessors (the chain is
-// transitive).  B200SEG_PDL=0 turns the attribute off (the device instructions are then no-ops).
+// transitive).
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_enter() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -161,21 +161,8 @@ __device__ __forceinline__ void pdl_enter() {
 // first, run the prologue, THEN wait -- the prologue overlaps the tail of the kernel before.  Nothing before
 // PDL_WAIT() may touch global memory: a chain of triggered kernels can be resident before ANY of them has completed,
 // so not even data written many launches ago (packed weights) is safe to read early.  Every thread executes the wait.
-#ifdef B200SEG_PDL_WAIT_FIRST      // A/B builds: wait before the prologue, as PDL_ENTER does
-#define PDL_TRIGGER() b200seg::pdl_enter()
-#define PDL_WAIT() ((void)0)
-#else
 #define PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 #define PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
-#endif
-
-inline bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200SEG_PDL");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
 
 template <typename... KArgs, typename... Args>
 inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -189,7 +176,7 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   (void)cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);     // errors surface in B200_LAUNCH_CHECK
 }
 

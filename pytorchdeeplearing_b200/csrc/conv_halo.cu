@@ -12,14 +12,11 @@
 //     SBO = 160 B (one halo row) apart and the two K-chunks LBO = one plane apart, for EVERY tap: the tap only
 //     moves the descriptor start address by (kh*10 + kw)*16 B inside the slice selected by kd;
 //   * the packed weights of all taps stay resident in smem for the CTA's lifetime;
-//   * loader warps move global -> registers -> smem with 128-bit accesses (this is where norm-on-load will be
-//     fused); the MMA warpgroup (two M64 halves, register accumulators), the double-buffered accumulator staging
-//     tile in shared memory and the epilogue (bias, GroupNorm statistics, residual addend, bf16 NDHWC stores)
-//     follow conv_tc.cu.
-// Warp roles (512 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue, warps 8-15 loaders
-// (software-pipelined: the loads of slice i+1 are in flight while slice i is stored).
-#include <stdlib.h>
-
+//   * loader warps move global -> smem with 16-byte cp.async (zero fill = conv padding); the MMA warpgroup (two
+//     M64 halves, register accumulators), the double-buffered accumulator staging tile in shared memory and the
+//     epilogue (bias, GroupNorm statistics, residual addend, bf16 NDHWC stores) follow conv_tc.cu.
+// conv_halo_kernel below is the 2-D (1x3x3) form; the 3-D layers take the input-slice-major conv_halo3_kernel.
+// Warp roles (512 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue, warps 8-15 loaders.
 #include "tc_common.cuh"
 
 namespace b200seg {
@@ -47,8 +44,6 @@ struct HaloArgs {
   int nitems;             // N * th * tw * ndchunks
   int nslices;            // ring size
   int acc_pitch;          // floats per row of the accumulator staging tile in shared memory
-  int swap_lbo_sbo;       // debug: swap the roles of the two descriptor strides
-  int cp_async;           // 1: loaders use cp.async (zfill) + mbarrier completion; 0: register-staged copies
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats): the output of this conv is
   // g = dL/d(act) of the layer whose raw output is yfwd; with m = [yfwd*A + B > 0] (A, B = that layer's GroupNorm /
   // dropout coefficients, derived here from its statistics exactly as gn_cta_coefs does) the epilogue accumulates
@@ -62,24 +57,14 @@ struct HaloArgs {
   int ggroups;
   double gm;              // elements per group
   float geps;
-  int exp;                // debug experiments (B200SEG_HALO_EXP bitmask): 1 no MMAs, 2 no epilogue work, 4 no loads
-  long long* dbg;         // debug timeline (B200SEG_HALO_DBG=1): [role 0..3][64 events] clock64 stamps of CTA 0
 };
-
-__device__ __forceinline__ void halo_stamp(const HaloArgs& p, int role, int idx) {
-  if (p.dbg != nullptr && blockIdx.x == 0 && idx < 64) {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.dbg[role * 64 + idx] = t;
-  }
-}
 
 __device__ __forceinline__ uint64_t make_nosw_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) |
          ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 
-template <int CIN, int COUT, int KD>
+template <int CIN, int COUT>
 __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloArgs p) {
   PDL_ENTER();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -87,7 +72,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
   constexpr int CP = CIN / 8;                                // 8-channel planes
   constexpr uint32_t PLANE = HP_H * HP_W * 16u;              // bytes of one plane of one slice
   constexpr uint32_t SLICE = (uint32_t)CP * PLANE;
-  constexpr int taps = KD * 9;
+  constexpr int taps = 9;
   constexpr uint32_t W_BYTES = (uint32_t)taps * CIN * COUT * 2u;
   uint8_t* s_w = smem;
   uint8_t* s_ring = smem + ((W_BYTES + 127u) & ~127u);
@@ -109,8 +94,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nslices; ++s) {
-      // register loader: one arrive per loader warp; cp.async loader: one (deferred) arrive per loader thread
-      mbar_init(&sfull[s], p.cp_async ? 32 * kLoaderWarps : kLoaderWarps);
+      mbar_init(&sfull[s], 32 * kLoaderWarps);   // one (deferred, cp.async) arrive per loader thread
       mbar_init(&sempty[s], 4);     // one arrive per MMA warp
     }
     for (int a = 0; a < 2; ++a) {
@@ -125,7 +109,6 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
   for (int i = threadIdx.x; i < 8 * p.Cout; i += blockDim.x) s_stat[i] = 0.f;
   fence_proxy_async();
   __syncthreads();
-  constexpr int pd = KD / 2;
 
   auto decode = [&](int item, int& n, int& h0, int& w0, int& d0, int& nd) {
     int t = item;
@@ -142,28 +125,18 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
   if (warp < 4) {
     // ===================================================== MMA warpgroup
     const int wt = threadIdx.x;
-    const uint32_t a_lbo = p.swap_lbo_sbo ? HP_W * 16u : PLANE;
-    const uint32_t a_sbo = p.swap_lbo_sbo ? PLANE : HP_W * 16u;
-    const uint32_t b_lbo = p.swap_lbo_sbo ? 128u : (uint32_t)COUT * 16u;
-    const uint32_t b_sbo = p.swap_lbo_sbo ? (uint32_t)COUT * 16u : 128u;
-    const uint64_t a_hi = make_nosw_desc(0, a_lbo, a_sbo);
-    const uint64_t b_hi = make_nosw_desc(0, b_lbo, b_sbo);
+    const uint64_t a_hi = make_nosw_desc(0, PLANE, HP_W * 16u);
+    const uint64_t b_hi = make_nosw_desc(0, (uint32_t)COUT * 16u, 128u);
     const uint32_t ring_u32 = smem_u32(s_ring);
     const uint64_t b_base = b_hi | (uint64_t)(smem_u32(s_w) >> 4);
     constexpr int kchunks = CIN / 16;
-    uint32_t gs = 0;   // slices consumed so far (ring position of the item's first slice)
-    uint32_t go = 0;   // output slice-tiles produced so far
+    uint32_t go = 0;   // output slice-tiles produced so far = input slices consumed (output o reads input slice o)
     for (int item = item_begin; item < item_end; ++item) {
       int n, h0, w0, d0, nd;
       decode(item, n, h0, w0, d0, nd);
-      const int nsl = nd + KD - 1;
       for (int o = 0; o < nd; ++o, ++go) {
-        // input slices o .. o+KD-1 of this item must have landed
-        const int first_wait = (o == 0) ? 0 : KD - 1;
-        for (int k = first_wait; k < KD; ++k) {
-          const uint32_t sl = gs + o + k;
-          mbar_wait(&sfull[sl % p.nslices], (sl / p.nslices) & 1u);
-        }
+        const uint32_t slot = go % p.nslices;
+        mbar_wait(&sfull[slot], (go / p.nslices) & 1u);
         const uint32_t as = go & 1u;
         // slices written by cp.async (generic proxy) must be ordered before the tensor core's async-proxy reads
         fence_proxy_async();
@@ -174,48 +147,36 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
         wgmma_fence_regs(acc1);
         wgmma_fence();
         {
-          // straight-line issue: every descriptor is (per-slice base) + compile-time offset, in 16-byte units;
+          // straight-line issue: every descriptor is (slice base) + compile-time offset, in 16-byte units;
           // rows 64..127 of the tile (hh = 8..15) start 8 halo rows further on
+          const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + slot * SLICE) >> 4);
 #pragma unroll
-          for (int kd_ = 0; kd_ < KD; ++kd_) {
-            const uint32_t sl = gs + o + kd_;
-            const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % p.nslices) * SLICE) >> 4);
+          for (int kh_ = 0; kh_ < 3; ++kh_)
 #pragma unroll
-            for (int kh_ = 0; kh_ < 3; ++kh_)
+            for (int kw_ = 0; kw_ < 3; ++kw_)
 #pragma unroll
-              for (int kw_ = 0; kw_ < 3; ++kw_)
-#pragma unroll
-                for (int kc = 0; kc < kchunks; ++kc) {
-                  constexpr uint32_t dummy = 0;
-                  (void)dummy;
-                  const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)(kh_ * HP_W + kw_) * 16u) >> 4;
-                  const uint32_t b_off = ((uint32_t)((((kd_ * 3 + kh_) * 3 + kw_) * kchunks + kc) * 2 * COUT) * 16u) >> 4;
-                  Wgmma<COUT, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
-                  Wgmma<COUT, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);
-                }
-          }
+              for (int kc = 0; kc < kchunks; ++kc) {
+                const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)(kh_ * HP_W + kw_) * 16u) >> 4;
+                const uint32_t b_off = ((uint32_t)(((kh_ * 3 + kw_) * kchunks + kc) * 2 * COUT) * 16u) >> 4;
+                Wgmma<COUT, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
+                Wgmma<COUT, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);
+              }
         }
         wgmma_commit();
         wgmma_wait0();
         wgmma_fence_regs(acc0);
         wgmma_fence_regs(acc1);
         __syncwarp();
-        if (lane == 0) {
-          // input slice o is no longer needed; at the end of the item neither are the trailing KD-1
-          mbar_arrive(&sempty[(gs + o) % p.nslices]);
-          if (o == nd - 1)
-            for (int k = 1; k < KD; ++k) mbar_arrive(&sempty[(gs + o + k) % p.nslices]);
-        }
+        if (lane == 0) mbar_arrive(&sempty[slot]);   // input slice o is no longer needed
         mbar_wait(&tempty[as], ((go >> 1) & 1u) ^ 1u);
         frag_store(s_acc + as * COUT, p.acc_pitch, 0, acc0, wt);
         frag_store(s_acc + as * COUT, p.acc_pitch, 64, acc1, wt);
         __syncwarp();
         if (lane == 0) mbar_arrive(&tfull[as]);
       }
-      gs += (uint32_t)nsl;
     }
   } else if (warp >= 8) {
-    // ===================================================== loaders (8 warps, software pipelined)
+    // ===================================================== loaders (8 warps)
     constexpr int LT = 32 * kLoaderWarps;
     const int lt = threadIdx.x - 256;
     const int pieces = HP_H * HP_W * CP;
@@ -235,86 +196,36 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
       pww[j] |= plane << 16;
     }
     // iterator over (item, slice)
-    int it_item = item_begin, it_i = 0, it_nsl = 0, n = 0, h0 = 0, w0 = 0, d0 = 0, nd = 0;
-    if (it_item < item_end) {
-      decode(it_item, n, h0, w0, d0, nd);
-      it_nsl = nd + KD - 1;
-    }
-    uint4 regs[kMaxPieces];
-    auto issue_loads = [&]() {
-      const int d = d0 - pd + it_i;
-      const bool dok = (unsigned)d < (unsigned)p.D;
-      const bf16* src = p.x + (((long long)n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
-#pragma unroll
-      for (int j = 0; j < kMaxPieces; ++j) {
-        const int plane = pww[j] >> 16, ww = pww[j] & 0xffff;
-        const int h = h0 - 1 + phh[j], w = w0 - 1 + ww;
-        uint4 val = make_uint4(0u, 0u, 0u, 0u);
-        if (pval[j] && dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W)
-          val = *reinterpret_cast<const uint4*>(src + ((long long)h * p.W + w) * p.xld + plane * 8);
-        regs[j] = val;
-      }
-    };
+    int it_item = item_begin, it_i = 0, n = 0, h0 = 0, w0 = 0, d0 = 0, nd = 0;
+    if (it_item < item_end) decode(it_item, n, h0, w0, d0, nd);
+    // fully asynchronous: as many slices in flight as the ring has free slots
     uint32_t sl = 0;
-    if (p.cp_async) {
-      // fully asynchronous: as many slices in flight as the ring has free slots
-      while (it_item < item_end) {
-        const uint32_t slot = sl % p.nslices;
-        mbar_wait(&sempty[slot], ((sl / p.nslices) & 1u) ^ 1u);
-        const uint32_t dst = smem_u32(s_ring + (size_t)slot * SLICE);
-        const int d = d0 - pd + it_i;
-        const bool dok = (unsigned)d < (unsigned)p.D;
-        const bf16* src = p.x + (((long long)n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
-#pragma unroll
-        for (int j = 0; j < kMaxPieces; ++j) {
-          if (!pval[j]) continue;
-          const int plane = pww[j] >> 16, ww = pww[j] & 0xffff;
-          const int h = h0 - 1 + phh[j], w = w0 - 1 + ww;
-          const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
-          const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)poff[j]), "l"(g),
-                       "r"(ok ? 16 : 0)
-                       : "memory");
-        }
-        asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&sfull[slot])) : "memory");
-        ++it_i;
-        if (it_i == it_nsl) {
-          ++it_item;
-          it_i = 0;
-          if (it_item < item_end) {
-            decode(it_item, n, h0, w0, d0, nd);
-            it_nsl = nd + KD - 1;
-          }
-        }
-        ++sl;
-      }
-      asm volatile("cp.async.wait_all;" ::: "memory");
-    } else {
-    if (it_item < item_end) issue_loads();
     while (it_item < item_end) {
       const uint32_t slot = sl % p.nslices;
       mbar_wait(&sempty[slot], ((sl / p.nslices) & 1u) ^ 1u);
-      uint8_t* dst = s_ring + (size_t)slot * SLICE;
+      const uint32_t dst = smem_u32(s_ring + (size_t)slot * SLICE);
+      const bf16* src = p.x + (((long long)n * p.D + d0 + it_i) * p.H) * p.W * p.xld;
 #pragma unroll
-      for (int j = 0; j < kMaxPieces; ++j)
-        if (pval[j]) *reinterpret_cast<uint4*>(dst + poff[j]) = regs[j];
-      // advance and put the next slice's loads in flight before signalling this one
+      for (int j = 0; j < kMaxPieces; ++j) {
+        if (!pval[j]) continue;
+        const int plane = pww[j] >> 16, ww = pww[j] & 0xffff;
+        const int h = h0 - 1 + phh[j], w = w0 - 1 + ww;
+        const bool ok = (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
+        const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)poff[j]), "l"(g),
+                     "r"(ok ? 16 : 0)
+                     : "memory");
+      }
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&sfull[slot])) : "memory");
       ++it_i;
-      if (it_i == it_nsl) {
+      if (it_i == nd) {
         ++it_item;
         it_i = 0;
-        if (it_item < item_end) {
-          decode(it_item, n, h0, w0, d0, nd);
-          it_nsl = nd + KD - 1;
-        }
+        if (it_item < item_end) decode(it_item, n, h0, w0, d0, nd);
       }
-      fence_proxy_async();            // generic-proxy stores -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sfull[slot]);
-      if (it_item < item_end) issue_loads();
       ++sl;
     }
-    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
   } else {
     // ===================================================== epilogue warps 4..7
     const int q = warp & 3;
@@ -465,8 +376,8 @@ __device__ __forceinline__ void halo3_mma(float* acc, int pitch, uint64_t a_base
 }
 constexpr int kHaloDepth = 6;          // cp.async groups (slices) in flight per loader thread; must be < ring slices
 
-template <int CIN, int COUT, int NCTA, bool BWD>
-__global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const HaloArgs p) {
+template <int CIN, int COUT, bool BWD>
+__global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArgs p) {
   PDL_TRIGGER();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
@@ -513,7 +424,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
   // the accumulator ring starts at zero (every MMA accumulates)
   for (int i = threadIdx.x; i < 128 * p.acc_pitch; i += blockDim.x) s_acc[i] = 0.f;
   __syncthreads();
-  if (threadIdx.x == 0) halo_stamp(p, 0, 63);
   // everything above is on-chip set-up and runs under the tail of the previous kernel; global memory from here on
   PDL_WAIT();
   // resident weights: 16-byte granules of the packed image [tap = (kd,kh,kw)][plane][co] -> [(kh,kw)][plane][2-kd][co]
@@ -559,7 +469,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
       for (int i = 0; i < nsl; ++i) {
         const uint32_t sl = gs + (uint32_t)i;
         mbar_wait(&sfull[sl % p.nslices], (sl / p.nslices) & 1u);
-        if (wt == 0) halo_stamp(p, 0, (int)sl);
         if (i < nd) {
           // output i is touched for the first time: its slot must have been drained (and zeroed) by the epilogue
           const uint32_t gn_ = go + (uint32_t)i;
@@ -580,11 +489,9 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
             float* acc = s_acc + slot0 * COUT;
             const uint32_t row0 = (uint32_t)(2 - i + o0) * COUT;            // weight rows: kd = i - o  ->  (2 - kd) * Cout
             const uint64_t b_base = b_hi | (uint64_t)((w_u32 + row0 * 16u) >> 4);
-            if (!(p.exp & 1)) {
-              if (cnt == 1) halo3_mma<CIN, COUT, COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-              else if (cnt == 2) halo3_mma<CIN, COUT, 2 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-              else halo3_mma<CIN, COUT, 3 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-            }
+            if (cnt == 1) halo3_mma<CIN, COUT, COUT>(acc, p.acc_pitch, a_base, b_base, wt);
+            else if (cnt == 2) halo3_mma<CIN, COUT, 2 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
+            else halo3_mma<CIN, COUT, 3 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
             o0 += cnt;
           }
           __syncwarp();
@@ -592,7 +499,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
             if (i >= 2) mbar_arrive(&tfull[(go + (uint32_t)(i - 2)) % R]);   // output i-2 has all three contributions
             mbar_arrive(&sempty[sl % p.nslices]);                            // this input slice is consumed
           }
-          if (wt == 0) halo_stamp(p, 1, (int)sl);
         }
       }
       gs += (uint32_t)nsl;
@@ -636,38 +542,29 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
       const int d = d0 - pd + it_i;
       const bool dok = (unsigned)d < (unsigned)p.D;
       const bf16* src = p.x + (((long long)n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
-      if (!(p.exp & 4)) {
 #pragma unroll 4
-        for (int q = lane; q < pieces; q += 32) {
-          const int v = q / CP, plane = q - v * CP;
-          const int hh = v / HP_W, ww = v - hh * HP_W;
-          const int h = h0 - 1 + hh, w = w0 - 1 + ww;
-          const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
-          const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
-                       "l"(g), "r"(ok ? 16 : 0)
-                       : "memory");
-        }
+      for (int q = lane; q < pieces; q += 32) {
+        const int v = q / CP, plane = q - v * CP;
+        const int hh = v / HP_W, ww = v - hh * HP_W;
+        const int h = h0 - 1 + hh, w = w0 - 1 + ww;
+        const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
+        const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
+                     "l"(g), "r"(ok ? 16 : 0)
+                     : "memory");
       }
       asm volatile("cp.async.commit_group;" ::: "memory");
-      if (lane == 0) halo_stamp(p, 2, (int)sl);
-      if (NCTA == 2) {
-        // two CTAs per SM, 4-8 slice ring: one slice in flight per warp (eight per SM)
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        signal(sl);
-      } else {
-        // one CTA per SM, deep ring: two cp.async groups in flight per warp; signal the older one
-        if (have_prev) {
-          asm volatile("cp.async.wait_group 1;" ::: "memory");
-          signal(prev_sl);
-        }
-        prev_sl = sl;
-        have_prev = true;
+      // two cp.async groups in flight per warp; signal the older one
+      if (have_prev) {
+        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        signal(prev_sl);
       }
+      prev_sl = sl;
+      have_prev = true;
       advance(kH3Loaders);
       sl += kH3Loaders;
     }
-    if (NCTA != 2 && have_prev) {
+    if (have_prev) {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
       signal(prev_sl);
     }
@@ -771,7 +668,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
         }
         const uint32_t as = go % R;
         mbar_wait(&tfull[as], (go / R) & 1u);
-        if (etid == 0) halo_stamp(p, 3, (int)go);
         float* tacc = s_acc + row * p.acc_pitch + as * COUT;
 #pragma unroll
         for (int c0 = 0; c0 < COUT; c0 += 16) {
@@ -785,7 +681,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
             __syncwarp();
             if (lane == 0) mbar_arrive(&tempty[as]);
           }
-          if (p.exp & 2) continue;
 #pragma unroll
           for (int j = 0; j < 16; j += 4) {
             const float4 b4 = *reinterpret_cast<const float4*>(s_bias + c0 + j);
@@ -891,9 +786,6 @@ __global__ void __launch_bounds__(kH3Threads, NCTA) conv_halo3_kernel(const Halo
     }
     if (want_stats && cur_n >= 0) flush_stats(cur_n);
   }
-
-  __syncthreads();
-  if (threadIdx.x == 0) halo_stamp(p, 1, 63);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -922,32 +814,22 @@ int conv_halo_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype
 
 static int g_halo_init[64] = {0};
 
-// 1 if conv_halo can fuse the GroupNorm-backward sums of the layer behind `y` into its epilogue (3-D layers only)
-int conv_halo_bwdstats_ok(int dims) {
-  static const int halo3 = [] {
-    const char* e = getenv("B200SEG_HALO3");
-    return (e && e[0] == '0') ? 0 : 1;
-  }();
-  return halo3 && dims == 3;
-}
-
 int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, const float* bias, const b200seg_tensor* y,
               double* stats, const b200seg_tensor* addend, int device, cudaStream_t st, const b200seg_tensor* yfwd,
               const b200seg_gn* gn, double* sums) {
   (void)kind;
   const int maxsm = tc_max_smem(device);
   if (device >= 0 && device < 64 && !g_halo_init[device]) {
-#define HALO_ATTR(CI, CO, K) \
-  B200_CUDA(cudaFuncSetAttribute(conv_halo_kernel<CI, CO, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm))
-    HALO_ATTR(16, 16, 3); HALO_ATTR(16, 32, 3); HALO_ATTR(32, 16, 3); HALO_ATTR(32, 32, 3);
-    HALO_ATTR(16, 16, 1); HALO_ATTR(16, 32, 1); HALO_ATTR(32, 16, 1); HALO_ATTR(32, 32, 1);
+#define HALO_ATTR(CI, CO) \
+  B200_CUDA(cudaFuncSetAttribute(conv_halo_kernel<CI, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm))
+    HALO_ATTR(16, 16); HALO_ATTR(16, 32); HALO_ATTR(32, 16); HALO_ATTR(32, 32);
 #undef HALO_ATTR
-#define HALO3_ATTR(CI, CO, NC) \
-  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm)); \
-  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)); \
-  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm)); \
-  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, NC, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100))
-    HALO3_ATTR(16, 16, 1); HALO3_ATTR(16, 32, 1); HALO3_ATTR(32, 16, 1); HALO3_ATTR(32, 32, 1);
+#define HALO3_ATTR(CI, CO) \
+  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm)); \
+  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)); \
+  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm)); \
+  B200_CUDA(cudaFuncSetAttribute(conv_halo3_kernel<CI, CO, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100))
+    HALO3_ATTR(16, 16); HALO3_ATTR(16, 32); HALO3_ATTR(32, 16); HALO3_ATTR(32, 32);
 #undef HALO3_ATTR
     g_halo_init[device] = 1;
   }
@@ -965,7 +847,7 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   p.yfwd = nullptr; p.yfld = 0; p.gstats = nullptr; p.ggamma = nullptr; p.gbeta = nullptr; p.gscale = nullptr;
   p.ggroups = 1; p.gm = 1.0; p.geps = 0.f;
   if (yfwd != nullptr) {
-    B200_CHECK_ARG(conv_halo_bwdstats_ok(dims) && gn != nullptr && sums != nullptr && stats == nullptr,
+    B200_CHECK_ARG(dims == 3 && gn != nullptr && sums != nullptr && stats == nullptr,
                    "conv_halo: backward statistics need the 3-D input-slice-major kernel");
     B200_CHECK_ARG(same_geom(yfwd, y) && yfwd->dtype == B200SEG_BF16 && (yfwd->ld % 8) == 0 && al16h(yfwd->ptr) &&
                        gn->groups > 0 && (y->c % gn->groups) == 0 && gn->groups <= 8,
@@ -982,18 +864,19 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   p.th = (p.H + HT_H - 1) / HT_H;
   const int cols = p.N * p.th * p.tw;
   const int sms = num_sms(device);
-  static const int halo3 = [] {
-    const char* e = getenv("B200SEG_HALO3");
-    return (e && e[0] == '0') ? 0 : 1;            // input-slice-major kernel for the 3-D layers (default on)
-  }();
-  const bool use3 = halo3 && p.kd == 3;
   // split d so that the grid covers the chip (each extra chunk re-loads kd-1 halo slices); one CTA per SM with a
   // deep slice ring
   const uint32_t slice = (uint32_t)(p.Cin / 8) * HP_H * HP_W * 16u;
   const uint32_t wbytes = ((uint32_t)(p.kd * 9) * p.Cin * p.Cout * 2u + 127u) & ~127u;
-  p.acc_pitch = (use3 ? kAccRing : 2) * p.Cout + 4;
-  const uint32_t tail = (2 * kHaloMaxSlices + (use3 ? 2 * kAccRing : 4)) * 8 + 16 + (use3 ? 11 : 8) * p.Cout * 4 + 64 +
-                        (use3 ? (2 * p.Cout + 16) * 8 + 8 : 0) + 16 + 128u * (uint32_t)p.acc_pitch * 4u;
+  uint32_t tail;
+  if (p.kd == 3) {
+    p.acc_pitch = kAccRing * p.Cout + 4;
+    tail = (2 * kHaloMaxSlices + 2 * kAccRing) * 8 + 16 + 11 * p.Cout * 4 + 64 + (2 * p.Cout + 16) * 8 + 8 + 16 +
+           128u * (uint32_t)p.acc_pitch * 4u;
+  } else {
+    p.acc_pitch = 2 * p.Cout + 4;
+    tail = (2 * kHaloMaxSlices + 4) * 8 + 16 + 8 * p.Cout * 4 + 64 + 16 + 128u * (uint32_t)p.acc_pitch * 4u;
+  }
   const int slots = sms;
   int ndch = 1;
   if (cols < slots) {
@@ -1009,70 +892,27 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   if (ns > kHaloMaxSlices) ns = kHaloMaxSlices;
   B200_CHECK_ARG(ns >= p.kd + 1, "conv_halo: slices do not fit in shared memory");
   p.nslices = ns;
-  static const int swap = [] {
-    const char* e = getenv("B200SEG_HALO_SWAP");
-    return (e && e[0] == '1') ? 1 : 0;
-  }();
-  p.swap_lbo_sbo = swap;
-  static const int cpa = [] {
-    const char* e = getenv("B200SEG_HALO_LOADER");
-    return (e && e[0] == 'r') ? 0 : 1;          // "regs" selects the register-staged loader
-  }();
-  p.cp_async = cpa;
-  static const int exp_bits = [] {
-    const char* e = getenv("B200SEG_HALO_EXP");
-    return e ? atoi(e) : 0;
-  }();
-  p.exp = exp_bits;
-  p.dbg = nullptr;
-  static const int dbg_on = [] {
-    const char* e = getenv("B200SEG_HALO_DBG");
-    return (e && e[0] == '1') ? 1 : 0;
-  }();
-  static long long* dbg_buf = nullptr;
-  if (dbg_on) {               // development aid only: allocates and synchronises
-    if (dbg_buf == nullptr) cudaMalloc(&dbg_buf, 4 * 64 * sizeof(long long));
-    cudaMemsetAsync(dbg_buf, 0, 4 * 64 * sizeof(long long), st);
-    p.dbg = dbg_buf;
-  }
   const size_t smem_bytes = 128 + wbytes + (size_t)ns * slice + tail;
   int grid = slots < p.nitems ? slots : p.nitems;
-#define HALO_LAUNCH(CI, CO, K) launch_k(conv_halo_kernel<CI, CO, K>, grid, kHaloThreads, smem_bytes, st, p)
-#define HALO3_LAUNCH(CI, CO, NC)                                                                         \
+#define HALO_LAUNCH(CI, CO) launch_k(conv_halo_kernel<CI, CO>, grid, kHaloThreads, smem_bytes, st, p)
+#define HALO3_LAUNCH(CI, CO)                                                                             \
   do {                                                                                                   \
-    if (p.yfwd != nullptr) launch_k(conv_halo3_kernel<CI, CO, NC, true>, grid, kH3Threads, smem_bytes, st, p);  \
-    else launch_k(conv_halo3_kernel<CI, CO, NC, false>, grid, kH3Threads, smem_bytes, st, p);            \
+    if (p.yfwd != nullptr) launch_k(conv_halo3_kernel<CI, CO, true>, grid, kH3Threads, smem_bytes, st, p);  \
+    else launch_k(conv_halo3_kernel<CI, CO, false>, grid, kH3Threads, smem_bytes, st, p);                \
   } while (0)
-  if (use3) {
-    if (p.Cin == 16 && p.Cout == 16) HALO3_LAUNCH(16, 16, 1);
-    else if (p.Cin == 16) HALO3_LAUNCH(16, 32, 1);
-    else if (p.Cout == 16) HALO3_LAUNCH(32, 16, 1);
-    else HALO3_LAUNCH(32, 32, 1);
-  } else if (p.kd == 3) {
-    if (p.Cin == 16 && p.Cout == 16) HALO_LAUNCH(16, 16, 3);
-    else if (p.Cin == 16) HALO_LAUNCH(16, 32, 3);
-    else if (p.Cout == 16) HALO_LAUNCH(32, 16, 3);
-    else HALO_LAUNCH(32, 32, 3);
+  if (p.kd == 3) {
+    if (p.Cin == 16 && p.Cout == 16) HALO3_LAUNCH(16, 16);
+    else if (p.Cin == 16) HALO3_LAUNCH(16, 32);
+    else if (p.Cout == 16) HALO3_LAUNCH(32, 16);
+    else HALO3_LAUNCH(32, 32);
   } else {
-    if (p.Cin == 16 && p.Cout == 16) HALO_LAUNCH(16, 16, 1);
-    else if (p.Cin == 16) HALO_LAUNCH(16, 32, 1);
-    else if (p.Cout == 16) HALO_LAUNCH(32, 16, 1);
-    else HALO_LAUNCH(32, 32, 1);
+    if (p.Cin == 16 && p.Cout == 16) HALO_LAUNCH(16, 16);
+    else if (p.Cin == 16) HALO_LAUNCH(16, 32);
+    else if (p.Cout == 16) HALO_LAUNCH(32, 16);
+    else HALO_LAUNCH(32, 32);
   }
 #undef HALO_LAUNCH
 #undef HALO3_LAUNCH
-  if (dbg_on && use3) {
-    long long h[4 * 64];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, dbg_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    const long long t0 = h[63];
-    fprintf(stderr, "[halo3 dbg] Cin=%d Cout=%d D=%d H=%d W=%d items=%d dchunk=%d ns=%d  end=%lld ns\n", p.Cin, p.Cout, p.D, p.H,
-            p.W, p.nitems, p.dchunk, p.nslices, h[64 + 63] - t0);
-    for (int i = 0; i < 40; ++i)
-      fprintf(stderr, "  sl %2d: load_issued %7lld  mma_sees_full %7lld  mma_issued %7lld | out %2d epi_sees_full %7lld\n", i,
-              h[128 + i] ? h[128 + i] - t0 : -1, h[i] ? h[i] - t0 : -1, h[64 + i] ? h[64 + i] - t0 : -1, i,
-              h[192 + i] ? h[192 + i] - t0 : -1);
-  }
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }

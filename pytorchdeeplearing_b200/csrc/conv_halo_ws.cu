@@ -15,8 +15,6 @@
 // Items = samples x columns x ceil(D / NACC) x (Cout / NT), so even the 12^3 level spreads over ~100 CTAs.
 // Warp roles (544 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue (bias, GroupNorm statistics, residual
 // addend, bf16 NDHWC stores), warps 8-15 slice loaders (cp.async, zero fill), warp 16 weight streamer.
-#include <stdlib.h>
-
 #include "tc_common.cuh"
 
 namespace b200seg {
@@ -56,16 +54,7 @@ struct HaloWsArgs {
   int ggroups;
   double gm;
   float geps;
-  unsigned long long* dbg;   // development aid: %globaltimer stamps of CTA 0 (null in production)
 };
-
-__device__ __forceinline__ void ws_stamp(const HaloWsArgs& p, int slot) {
-  if (p.dbg != nullptr && blockIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    p.dbg[slot] = t;
-  }
-}
 
 __device__ __forceinline__ uint64_t ws_nosw_desc(uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
@@ -99,7 +88,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) ws_stamp(p, 0);
 
   const int items_per_cta = (p.nitems + gridDim.x - 1) / gridDim.x;
   const int item_begin = blockIdx.x * items_per_cta;
@@ -124,7 +112,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
   fence_proxy_async();
   __syncthreads();
   PDL_WAIT();               // barriers and the statistics rows are set up under the tail of the previous kernel
-  if (threadIdx.x == 0) ws_stamp(p, 1);
 
   // item -> (sample, column, first output slice, slices, channel group); the channel group is the fastest index
   auto decode = [&](int item, int& n, int& h0, int& w0, int& d0, int& nd, int& ng) {
@@ -172,7 +159,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       for (int kd_ = 0; kd_ < 3; ++kd_) {
         if (kd_ == 0) {
           for (int k = 0; k < nd; ++k) wait_slice(k);
-          if (gi == 0 && wt == 0) ws_stamp(p, 2);
         } else {
           wait_slice(nd - 1 + kd_);
         }
@@ -217,7 +203,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
             if (lane == 0) mbar_arrive(&wempty[stg]);
           }
       }
-      if (gi == 0 && wt == 0) ws_stamp(p, 3);
       __syncwarp();
       if (lane == 0) {
 #pragma unroll
@@ -369,7 +354,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       const int cbase = ng * NT;
       const uint32_t as = gi % (uint32_t)p.accslots;
       mbar_wait(&tfull[as], (gi / (uint32_t)p.accslots) & 1u);
-      if (etid == 0 && gi == 0) ws_stamp(p, 4);
       const float* tacc = s_acc + row * p.acc_pitch + as * (NACC * NT);
       // GroupNorm statistics: per-thread (row) partials over the item's tiles, ONE warp fold per 16-column chunk
       // and item (chunk-outer order keeps only one chunk's partials in registers)
@@ -447,7 +431,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
         }
         if (c == NT / 16 - 1) {
           // the accumulators are drained: hand them back before the last (register-only) statistics fold
-          if (etid == 0 && gi == 0) ws_stamp(p, 5);
           __syncwarp();
           if (lane == 0) mbar_arrive(&tempty[as]);
         }
@@ -478,9 +461,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     }
     if (p.stats != nullptr && cur_n >= 0) flush_stats(cur_n);
   }
-
-  __syncthreads();
-  if (threadIdx.x == 0) ws_stamp(p, 6);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -581,11 +561,6 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
     p.gm = (double)(y->c / gn->groups) * (double)gn->vox;
     p.geps = gn->eps;
     p.stats = sums;
-  }
-  {
-    // B200SEG_WS_DBG=<device pointer, hex>: 8 x u64 time stamps of CTA 0 (tools/ws_timeline.py)
-    const char* e = getenv("B200SEG_WS_DBG");
-    p.dbg = e ? reinterpret_cast<unsigned long long*>(strtoull(e, nullptr, 16)) : nullptr;
   }
   // NT = 64 columns per MMA (narrower groups re-read A for less work); NACC = 1 keeps the warpgroup at 64
   // accumulator registers per thread, within the budget of a 544-thread CTA

@@ -589,7 +589,9 @@ int conv_tc(int kind, int dims, const b200seg_tensor* x, const void* wpk, const 
     const int tiles = p.N * ((p.W + bw_ - 1) / bw_) * ((p.H + bh_ - 1) / bh_) * ((p.D + bd_ - 1) / bd_);
     const int sms = num_sms(device);
     const int kblocks = g.kd * g.kh * g.kw * (p.Cin / pick_bkc(p.Cin));
-    const char* e = getenv("B200SEG_TC_KSPLIT");          // 0: off, n >= 2: at most n ranges, unset: automatic
+    // B200SEG_TC_KSPLIT (0: off, n >= 2: at most n ranges, unset: automatic) is read on every call: it is how the
+    // split-K test reaches the unsplit kernel on the same shape as its reference, and how it caps the ranges
+    const char* e = getenv("B200SEG_TC_KSPLIT");
     const int ks_max = e ? atoi(e) : 16;
     if (!g.up && kblocks >= 16 && ks_max >= 2) {
       int nt = p.Ntile, ngp = p.ngroups;
@@ -664,11 +666,7 @@ int conv_tc(int kind, int dims, const b200seg_tensor* x, const void* wpk, const 
   }
   int grid = num_sms(device);
   if (grid > p.ntiles * p.ngroups * p.ksplit) grid = p.ntiles * p.ngroups * p.ksplit;
-  static const bool regstats_off = [] {
-    const char* e = getenv("B200SEG_TC_REGSTATS");
-    return e && e[0] == '0';
-  }();
-  const int nch = regstats_off ? 0 : (p.Cout == 16 ? 1 : (p.Cout == 32 ? 2 : 0));
+  const int nch = p.Cout == 16 ? 1 : (p.Cout == 32 ? 2 : 0);
 #define TC_LAUNCH(B)                                                                         \
   do {                                                                                       \
     if (nch == 1) launch_k(conv_tc_kernel<B, 1>, grid, kTcThreads, smem_bytes, st, tmA, tmB, p);          \

@@ -1243,9 +1243,8 @@ int ew_gn_bwd_reduce(const b200seg_tensor* g, const b200seg_tensor* y, const flo
   const int C = y->c;
   EW_DISPATCH(y, vok, {
     const int G = C / VEC;
-    // large streams: deeper load pipeline, two CTAs per SM (B200SEG_GN_REDUCE_DEEP=0: the two-trip loop everywhere)
-    static const bool deep_on = [] { const char* e = getenv("B200SEG_GN_REDUCE_DEEP"); return !(e && e[0] == '0'); }();
-    const bool deep = deep_on && V * G >= (long long)num_sms(device) * 2 * 256 * 8;
+    // large streams: deeper load pipeline, two CTAs per SM
+    const bool deep = V * G >= (long long)num_sms(device) * 2 * 256 * 8;
     dim3 grid(ew_blocks(V, G, y->n, device, deep ? 2 : 3), y->n);
     const bool pow2g = (G & (G - 1)) == 0;
     const int groups = (gn && gn->stats) ? gn->groups : 1;

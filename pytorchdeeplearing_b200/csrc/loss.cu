@@ -8,8 +8,6 @@
 // (model/metric.py:146-181 dice_coeff / iou_coeff / multiclass_dice_coeff on the thresholded probabilities), so the
 // training step needs no separate read of ``probs`` for it, and counts labels outside [0, C) (the reference raises
 // in F.one_hot / F.cross_entropy; here the count lands in ``part`` and the host raises).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace b200seg {
@@ -473,10 +471,8 @@ static int loss_blocks(long long nvox_, int device) {
 // blocks per sample for the (blocks, N) grids of the partial-sum kernels
 static dim3 sample_grid(long long vox, int N, int device) {
   // blocks per SM over the whole grid: every block ends in one fp64 atomic per partial sum (15 for two classes) on
-  // the SAME few addresses, so more blocks buy load parallelism and pay in serialised atomics (B200SEG_LOSS_BPS)
-  const char* e = getenv("B200SEG_LOSS_BPS");          // read per call (host side, once per launch): in-process A/B
-  const int v = e ? atoi(e) : 0;
-  const int bps = v >= 1 && v <= 16 ? v : 4;
+  // the SAME few addresses, so more blocks buy load parallelism and pay in serialised atomics
+  const int bps = 4;
   long long per = (vox + 256 * 4 - 1) / (256 * 4);
   long long cap = ((long long)num_sms(device) * bps + N - 1) / N;
   if (per > cap) per = cap;

@@ -11,8 +11,6 @@
 //     (m16n8k16, fp32 accumulators);
 //   * epilogue on the accumulator fragments: + bias, GroupNorm statistics (per-lane column partials, folded once per
 //     sample), + addend, bf16x2 stores.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace b200seg {
@@ -207,23 +205,11 @@ __global__ void __launch_bounds__(PW_THREADS, UP ? 1 : 2)
 // ------------------------------------------------------------------------------------------------
 static bool al16pw(const void* p) { return (reinterpret_cast<uintptr_t>(p) % 16) == 0; }
 
-static const bool g_pw_off = [] {
-  const char* e = getenv("B200SEG_DISABLE_PW_MMA");
-  return e && e[0] == '1';
-}();
-
-static const bool g_pw_up_off = [] {
-  const char* e = getenv("B200SEG_PW_UP");
-  return e && e[0] == '0';
-}();
-
 static bool pw_ch(int c) { return c == 16 || c == 32 || c == 64; }
 
 int pw_mma_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                      const b200seg_tensor* addend) {
-  if (g_pw_off) return 0;
   if ((kind != B200SEG_K1 && kind != B200SEG_UP) || w_dtype != B200SEG_BF16_TC) return 0;
-  if (kind == B200SEG_UP && g_pw_up_off) return 0;
   if (!pw_ch(x->c) || !pw_ch(y->c)) return 0;
   if (x->c * y->c > (kind == B200SEG_UP ? 512 : 2048)) return 0;      // the weight fragments live in registers
   if (x->dtype != B200SEG_BF16 || y->dtype != B200SEG_BF16) return 0;

@@ -14,8 +14,6 @@
 //                        in the loop); the block folds its accumulators once at the end.
 //
 // smallcin (small_channels.cu) remains the fallback for Cin in 2..4 and odd widths.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace b200seg {
@@ -251,13 +249,8 @@ template <typename TX, typename TW, typename TY, int CO>
 static int stem_conv_co(int kind, int dims, const b200seg_tensor* x, const void* w, const float* bias,
                         const b200seg_tensor* y, double* stats, int device, cudaStream_t st) {
   // voxels per thread along w: 2 shares the input window between neighbours but needs the registers (it spills
-  // under the 2-CTA/SM bound for the 27-tap case); B200SEG_STEM_VPT=1|2 overrides for experiments
-  static const int vpt_env = [] {
-    const char* e = getenv("B200SEG_STEM_VPT");
-    return e ? atoi(e) : 0;
-  }();
+  // under the 2-CTA/SM bound for the 27-tap case)
   int vpt = (kind == B200SEG_K1 || dims == 2) ? 2 : 1;
-  if (vpt_env == 1 || vpt_env == 2) vpt = vpt_env;
   if (x->w & 1) vpt = 1;
   const long long items = (long long)x->d * x->h * (x->w / vpt);
   long long blocks = (items + 255) / 256;

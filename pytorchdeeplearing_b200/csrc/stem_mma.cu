@@ -14,8 +14,6 @@
 // ~16 LDS.U16 + 4 MMAs, so the kernels run at the speed of their HBM streams (image in, activations out / dY in).
 // Bias, GroupNorm statistics (fixed order: lanes -> warps -> one fp64 atomic per CTA and sample) and the bf16
 // NDHWC stores are fused into the forward epilogue.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace b200seg {
@@ -416,14 +414,8 @@ static bool stem_mma_geom(const b200seg_tensor* x, const b200seg_tensor* y, Stem
   return true;
 }
 
-static const bool g_stem_mma_off = [] {
-  const char* e = getenv("B200SEG_DISABLE_STEM_MMA");
-  return e && e[0] == '1';
-}();
-
 int stem_mma_conv_supported(int kind, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                             const b200seg_tensor* addend) {
-  if (g_stem_mma_off) return 0;
   if (kind != B200SEG_K3 && kind != B200SEG_K1) return 0;
   if (addend != nullptr || w_dtype != B200SEG_BF16 || y->dtype != B200SEG_BF16) return 0;
   if (x->dtype != B200SEG_F32 && x->dtype != B200SEG_BF16) return 0;
@@ -474,7 +466,6 @@ int stem_mma_conv(int kind, int dims, const b200seg_tensor* x, const void* w, co
 }
 
 int stem_mma_wgrad_supported(int kind, const b200seg_tensor* a, const b200seg_tensor* b) {
-  if (g_stem_mma_off) return 0;
   if (kind != B200SEG_K3 && kind != B200SEG_K1) return 0;
   if (b->dtype != B200SEG_BF16) return 0;
   if (a->dtype != B200SEG_F32 && a->dtype != B200SEG_BF16) return 0;

@@ -13,8 +13,6 @@
 //     fit), stream s owns every S-th 16-voxel group of the tile: warps = (27 / TPW) x S, all reading the same tile;
 //   * tiles are double buffered with cp.async (zero fill = conv padding); a CTA walks a contiguous tile range and
 //     folds its accumulators once at the end: streams through shared memory, then one fp32 atomic per weight.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace b200seg {
@@ -188,11 +186,6 @@ __global__ void __launch_bounds__(32 * (27 / TPW) * S, 1)
 // ------------------------------------------------------------------------------------------------
 static bool al16h2(const void* p) { return (reinterpret_cast<uintptr_t>(p) % 16) == 0; }
 
-static const bool g_wh_off = [] {
-  const char* e = getenv("B200SEG_DISABLE_WGRAD_HALO");
-  return e && e[0] == '1';
-}();
-
 static int wh_tile_w(int cin, int W) {
   const int want = cin == 16 ? 32 : 16;
   if (W % want == 0) return want;
@@ -201,7 +194,6 @@ static int wh_tile_w(int cin, int W) {
 }
 
 int wgrad_halo_mma_supported(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b) {
-  if (g_wh_off) return 0;
   if (kind != B200SEG_K3 || dims != 3) return 0;
   if (a->dtype != B200SEG_BF16 || b->dtype != B200SEG_BF16) return 0;
   if ((a->c != 16 && a->c != 32) || (b->c != 16 && b->c != 32)) return 0;

@@ -343,7 +343,7 @@ class Engine:
         vox = 1
         for s in out_sp:
             vox *= s
-        if getattr(self.be, "fused_gn", False) and cout <= 512:
+        if cout <= 512:
             # kernels derive the coefficients from the statistics themselves: no finalize launch
             # (wider layers -- init_features >= 64 -- take the finalize/apply form: any channel count)
             L.gn = (stats, self.P[gname + ".weight"], self.P[gname + ".bias"], L.scale, vox, GROUPS, GN_EPS)

@@ -69,8 +69,7 @@ class GraphedStep:
         if self._fused_opt:
             optimizer.prepare()
         self._plan = None
-        if (model.training and model.dropout_masks is None and x.is_cuda and runtime._TEST_BACKEND is None
-                and os.environ.get("B200SEG_PHILOX_MASKS", "1") != "0"):
+        if model.training and model.dropout_masks is None and x.is_cuda and runtime._TEST_BACKEND is None:
             self._plan = model.mask_plan(x.shape[0], dev)
         self._works = []
         self.loss = self.dice = self.probs = None

@@ -2,7 +2,6 @@
 the whole net to the layer program (``engine.Engine``), i.e. to the sm_90a kernels."""
 from __future__ import annotations
 
-import os
 import struct
 from typing import List, Optional
 
@@ -142,8 +141,7 @@ class SegNetBase(nn.Module):
             return None
         if self.dropout_masks is not None:
             return [m.to(device=x.device, dtype=torch.float32) for m in self.dropout_masks]
-        if (x.is_cuda and runtime._TEST_BACKEND is None and not runtime.is_capturing(x.device)
-                and os.environ.get("B200SEG_PHILOX_MASKS", "1") != "0"):
+        if x.is_cuda and runtime._TEST_BACKEND is None and not runtime.is_capturing(x.device):
             plan = self.mask_plan(x.shape[0], x.device)     # ONE launch instead of one bernoulli_ per layer
             plan.refresh()
             return plan.launch()

@@ -154,7 +154,6 @@ class EmuBackend:
         coef[..., 1] = ((b64 - mu_c * r_c * g64) * s).float()
 
     # fused-coefficient forms (composition of the unfused statements above)
-    fused_gn = True
 
     def _coef(self, gn, n, c):
         stats, gamma, beta, scale, vox, groups, eps = gn

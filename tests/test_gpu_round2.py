@@ -72,12 +72,9 @@ def test_philox_masks_equal_torch_per_module_draws(kind, n):
     for k, (a, b) in enumerate(zip(got, want)):
         assert torch.equal(a, b), k
     assert torch.equal(after, after_ref)                  # generator offset advanced identically
-    os.environ["B200SEG_PHILOX_MASKS"] = "0"
-    try:
-        torch.manual_seed(1234)
-        legacy = model._draw_masks(x)
-    finally:
-        del os.environ["B200SEG_PHILOX_MASKS"]
+    runtime._set_backend_for_testing(EmuBackend())       # the torch-draw branch (reset by the autouse fixture)
+    torch.manual_seed(1234)
+    legacy = model._draw_masks(x)
     assert all(torch.equal(a, b) for a, b in zip(legacy, want))
 
 

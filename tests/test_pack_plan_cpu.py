@@ -20,11 +20,9 @@ from pytorchdeeplearing_b200.engine import DOWN, K1, K3, UP
 from emu_backend import EmuBackend
 
 
-def _backend(use_tc=True):
+def _backend():
     be = object.__new__(_abi.CudaBackend)            # no CUDA device here: only the planning half of the backend
     be.lib = _abi.load_library()
-    be.use_tc = be.use_halo = be.use_halo_ws = use_tc
-    be.halo_min_vox, be.halo_ws_min_vox = 128 * 128, 1000
     return be
 
 
@@ -55,8 +53,9 @@ def test_cuda_core_layouts_equal_the_emulation_backend(kind, which, dims):
     """fp32 (parity mode) plans and bf16 plans with the tensor-core paths disabled"""
     w, a, b, taps = _weight(kind, 24, 40, dims)
     ref = EmuBackend().pack_weight(w, kind, which, torch.float32, dims)
-    for dtype, be in ((torch.float32, _backend()), (torch.bfloat16, _backend(use_tc=False))):
-        shape, code, args = be._pack_plan(w, kind, which, dtype, dims, True, 10 ** 6)
+    be = _backend()
+    for dtype, allow_tc in ((torch.float32, True), (torch.bfloat16, False)):
+        shape, code, args = be._pack_plan(w, kind, which, dtype, dims, allow_tc, 10 ** 6)
         assert code == (F32 if dtype == torch.float32 else BF16)
         got = _run_descs(w, shape, args)
         assert got.shape == ref.shape and torch.equal(got, ref)

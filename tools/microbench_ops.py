@@ -5,8 +5,7 @@
 Every op is timed with CUDA events on the current stream, once with a warm L2 (back-to-back launches) and
 once "cold" (a 256 MiB write between launches, the way bench.py flushes between steps).  This is a
 development tool: it prints a table and writes gpurun_out/microbench_<tag>.json; it is not a bench line.
-Environment switches of the library (B200SEG_DISABLE_STEM, B200SEG_STEM_VPT, ...) apply as usual, so two
-runs with different settings give an A/B comparison on the same box.
+B200SEG_LIB selects another build of the library, so two runs give an A/B comparison of two builds on the same box.
 """
 from __future__ import annotations
 

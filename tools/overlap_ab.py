@@ -1,14 +1,13 @@
 #!/usr/bin/env python
-"""A/B of the host-side scheduling options (B200SEG_OVERLAP bit mask, engine.py) and of the loss-pass grid
-(B200SEG_LOSS_BPS) on ONE box and in ONE process.  For every setting a fresh GraphedStep is captured on the same
+"""A/B of the host-side scheduling options (B200SEG_OVERLAP bit mask, engine.py) on ONE box and in ONE process.  For every setting a fresh GraphedStep is captured on the same
 model / inputs / dropout draw; its loss and gradients are compared with the first setting (same kernels on the same
 data: only atomic ordering may differ -- the list can repeat the baseline to show that noise floor) and the replay is
 timed like bench.py times it (device events, 256 MiB L2 flush before every step, median).
 
-  python tools/overlap_ab.py --masks 0,1,2,4,8,15,0 --bps 8,4,2 [--workload vnet3d|unet2d|unet3d] [--steps 30] \
+  python tools/overlap_ab.py --masks 0,1,2,4,8,15,0 [--workload vnet3d|unet2d|unet3d] [--steps 30] \
          [--choose gpurun_out/chosen_env.sh] >> gpurun_out/overlap_ab.jsonl
 
-``--choose FILE``: write ``export B200SEG_OVERLAP=..; export B200SEG_LOSS_BPS=..`` for the fastest setting whose
+``--choose FILE``: write ``export B200SEG_OVERLAP=..`` for the fastest setting whose
 results agree with the baseline (bits are kept when they gain on their own; the union must beat the baseline).
 """
 import argparse
@@ -29,12 +28,12 @@ GRAD_TOL = 2e-2        # relative L2 of the flat gradient against the baseline (
 MIN_GAIN_MS = 0.004    # a bit / grid setting is kept only for a median gain above the timing noise
 
 
-def select(measure, masks, bps_list):
-    """measure(mask, bps) -> record with "mask", "ms_median", "ok".  Returns (mask, bps or 0, summary or None)."""
-    recs = [measure(m, 0) for m in masks]
+def select(measure, masks):
+    """measure(mask) -> record with "mask", "ms_median", "ok".  Returns (mask, summary or None)."""
+    recs = [measure(m) for m in masks]
     base = [r for r in recs if r["mask"] == 0]
     if not base:
-        return 0, 0, None
+        return 0, None
     t0 = statistics.median([r["ms_median"] for r in base])
     keep = 0
     for bit in (1, 2, 4, 8):
@@ -46,29 +45,20 @@ def select(measure, masks, bps_list):
         if r["mask"] and r["ok"]:
             cands[r["mask"]] = min(cands.get(r["mask"], 1e9), r["ms_median"])
     if keep and keep not in cands:
-        r = measure(keep, 0)
+        r = measure(keep)
         if r["ok"]:
             cands[keep] = r["ms_median"]
-    chosen_mask, chosen_bps = 0, 0
+    chosen_mask = 0
     if cands:
         best = min(cands, key=cands.get)
         if t0 - cands[best] > MIN_GAIN_MS:
             chosen_mask = best
-    tb = cands.get(chosen_mask, t0)
-    for b in bps_list:
-        if b == 8:
-            continue
-        r = measure(chosen_mask, b)
-        if r["ok"] and tb - r["ms_median"] > MIN_GAIN_MS:
-            tb, chosen_bps = r["ms_median"], b
-    return chosen_mask, chosen_bps, {"baseline_ms": t0, "chosen_mask": chosen_mask, "chosen_bps": chosen_bps or 8,
-                                     "chosen_ms": tb}
+    return chosen_mask, {"baseline_ms": t0, "chosen_mask": chosen_mask, "chosen_ms": cands.get(chosen_mask, t0)}
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--masks", default="0,15")
-    ap.add_argument("--bps", default="")
     ap.add_argument("--workload", default="vnet3d")
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--choose", default="")
@@ -92,12 +82,8 @@ def main():
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
     ref = [None]
 
-    def measure(mask, bps):
+    def measure(mask):
         os.environ["B200SEG_OVERLAP"] = str(mask)
-        if bps:
-            os.environ["B200SEG_LOSS_BPS"] = str(bps)
-        else:
-            os.environ.pop("B200SEG_LOSS_BPS", None)
         step = GraphedStep(model, lossfn, x, y, warmup=2)
         for _ in range(5):
             step()
@@ -115,7 +101,7 @@ def main():
             evs.append((e0, e1))
         torch.cuda.synchronize()
         ms = [a.elapsed_time(b) for a, b in evs]
-        rec = {"workload": args.workload, "mask": mask, "bps": bps or 8, "ms_median": statistics.median(ms),
+        rec = {"workload": args.workload, "mask": mask, "ms_median": statistics.median(ms),
                "ms_min": min(ms), "ms_max": max(ms), "loss": loss, "grad_norm": float(flat.norm()),
                "finite": bool(torch.isfinite(flat).all()), "graphs": len(step.graphs)}
         if ref[0] is None:
@@ -132,16 +118,13 @@ def main():
         torch.cuda.empty_cache()
         return rec
 
-    chosen_mask, chosen_bps, summary = select(measure, [int(m) for m in args.masks.split(",")],
-                                              [int(v) for v in args.bps.split(",") if v])
+    chosen_mask, summary = select(measure, [int(m) for m in args.masks.split(",")])
     if summary is not None:
         summary["workload"] = args.workload
         print(json.dumps(summary), flush=True)
     if args.choose:
         with open(args.choose, "w") as f:
             f.write(f"export B200SEG_OVERLAP={chosen_mask}\n")
-            if chosen_bps:
-                f.write(f"export B200SEG_LOSS_BPS={chosen_bps}\n")
 
 
 if __name__ == "__main__":
