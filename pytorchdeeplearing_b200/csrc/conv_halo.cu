@@ -40,8 +40,8 @@ struct HaloArgs {
   int Cin, Cout;
   int kd;                 // 3 (3-D) or 1 (2-D)
   int tw, th;             // tiles along w, h
-  int dchunk, ndchunks;   // output slices per work item, items along d
-  int nitems;             // N * th * tw * ndchunks
+  int dchunk, ndchunks;   // 2-D kernel: output slices per work item, items along d
+  int nitems;             // 2-D kernel: N * th * tw * ndchunks
   int nslices;            // ring size
   int acc_pitch;          // floats per row of the accumulator staging tile in shared memory
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats): the output of this conv is
@@ -325,56 +325,62 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
 // ------------------------------------------------------------------------------------------------
 // Input-slice-major form of the 3-D kernel (KD = 3): every staged input slice is multiplied ONCE per (kh, kw, K chunk)
 // against the weights of all three kd taps side by side, B = [W(kd=2) | W(kd=1) | W(kd=0)] (N = 3*Cout columns), and
-// accumulates into the three output slices (i-2, i-1, i) it contributes to, which are neighbouring column ranges
-// of a ring of accumulators.  An MMA instruction re-reads its A operand (the voxel rows) from shared memory whatever
-// N is, so 9 instructions of N = 3*Cout per input slice instead of 27 of N = Cout per output slice do the same MACs
-// with a third of the A reads.
-//   * accumulators: ring of kAccRing slots of Cout columns; slot of output o = (running output count) % ring; an
-//     output is complete when the input slice two further on has been multiplied in (-> tfull[slot]);
-//   * all MMAs accumulate (one instruction spans the columns of up to three outputs): the epilogue reads a slot into
-//     registers, hands it back ZEROED at once and only then does its arithmetic; the whole ring is zeroed once at
-//     kernel start.
-//   * at the ends of an item's d-range the column range shrinks to the outputs that exist (N = Cout or 2*Cout,
-//     weight rows offset accordingly), and a range that would wrap around the ring is issued in two pieces;
+// accumulates into the three output slices (i-2, i-1, i) it contributes to.  An MMA instruction re-reads its A operand
+// (the voxel rows) from shared memory whatever N is, so 9 instructions of N = 3*Cout per input slice instead of 27 of
+// N = Cout per output slice do the same MACs with a third of the A reads.
+//   * work split: the output space is T = N * th * tw * D slice tiles ordered (n, h tile, w tile, d); CTA b of G owns
+//     [b*T/G, (b+1)*T/G) and walks it as column segments (n, h0, w0, d_a, nd).  A segment stages input slices
+//     d_a-1 .. d_a+nd (zero filled outside the volume).  All three roles take their segments from halo3_segment, so
+//     their slice and output sequences, and with them the mbarrier parities, agree;
+//   * accumulators: the MMA warpgroup holds the three outputs of the slice being multiplied in registers, 3*Cout/2
+//     fp32 per M64 half, in one fixed order: columns [0, Cout) output i-2, then i-1, then i.  A wgmma instruction
+//     takes its accumulator as one contiguous register range, so the three outputs cannot rotate in place from slice
+//     to slice (ptxas would copy them between the instructions and wait for each one); they shift down by one output
+//     per slice instead, 2*Cout register moves per thread;
+//   * every slice runs the full N = 3*Cout: at the ends of a segment the outputs before d_a and from d_a+nd on
+//     accumulate into columns that are zeroed before their first real use.  That keeps one instruction shape for
+//     2/(nd+2) extra tensor work, and every real output still sums exactly its three slices, in the same order, from
+//     zero;
+//   * the chain of slice i is waited for right after its issue (a wait further on, behind the mbarrier traffic, makes
+//     ptxas serialise every instruction of the chain); output i-2 is then complete and is written once to a
+//     double-buffered fp32 staging tile in shared memory (tfull / tempty, as in the 2-D kernel) for the epilogue;
+//   * registers per role (setmaxnreg): the loader warpgroup gives most of its share to the MMA warpgroup (three outputs'
+//     accumulators plus descriptors) and the epilogue (per-row GroupNorm sums of every channel);
 //   * the weight image in smem is the packed image permuted at load time to [(kh,kw)][Cin/8][kd reversed][Cout][8].
-// The accumulator ring lives in shared memory ([128 rows][ring * Cout] fp32): per input slice the MMA warpgroup
-// loads the columns of the outputs it contributes to into registers, runs the wgmma chain over them and stores them
-// back.  384 threads (4 MMA, 4 epilogue, 4 loader warps), one CTA per SM (two would leave 85 registers per thread).
+// 384 threads (4 MMA, 4 epilogue, 4 loader warps), one CTA per SM.
 // ------------------------------------------------------------------------------------------------
-constexpr int kAccRing = 4;
 constexpr int kH3Loaders = 4;          // loader warps of the input-slice-major kernel (warps 8..11)
 constexpr int kH3Threads = 32 * (4 + 4 + kH3Loaders);   // 384 threads
+// registers per thread after setmaxnreg; at 1 CTA of 384 threads each thread starts with 168 and the three roles
+// (one warpgroup each) may hold at most 3 * 168 between them
+constexpr uint32_t kH3RegsMma = 224, kH3RegsEpi = 224, kH3RegsLoad = 56;
+static_assert(kH3RegsMma + kH3RegsEpi + kH3RegsLoad <= 3 * 168, "register budget of conv_halo3_kernel");
 
-// one contiguous piece of the accumulator ring (N = outputs x Cout columns starting at `acc`) += one staged input
-// slice x the (kh, kw) weights of the matching kd taps, for the whole MMA warpgroup (wt = thread index inside it)
-template <int CIN, int COUT, int N>
-__device__ __forceinline__ void halo3_mma(float* acc, int pitch, uint64_t a_base, uint64_t b_base, int wt) {
-  constexpr int CP = CIN / 8;
-  constexpr uint32_t PLANE = HP_H * HP_W * 16u;
-  constexpr int kchunks = CIN / 16;
-  float acc0[N / 2], acc1[N / 2];
-  frag_load(acc, pitch, 0, acc0, wt);
-  frag_load(acc, pitch, 64, acc1, wt);
-  wgmma_fence_regs(acc0);
-  wgmma_fence_regs(acc1);
-  wgmma_fence();
-#pragma unroll
-  for (int t9 = 0; t9 < 9; ++t9)
-#pragma unroll
-    for (int kc = 0; kc < kchunks; ++kc) {
-      const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)((t9 / 3) * HP_W + (t9 % 3)) * 16u) >> 4;
-      const uint32_t b_off = ((uint32_t)(t9 * CP + 2 * kc) * 3u * COUT * 16u) >> 4;
-      Wgmma<N, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
-      Wgmma<N, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);   // rows 64..127: hh 8..15
-    }
-  wgmma_commit();
-  wgmma_wait0();
-  wgmma_fence_regs(acc0);
-  wgmma_fence_regs(acc1);
-  frag_store(acc, pitch, 0, acc0, wt);
-  frag_store(acc, pitch, 64, acc1, wt);
+// this CTA's share [begin, end) of the N * th * tw * D output slice tiles
+__device__ __forceinline__ void halo3_range(const HaloArgs& p, int& begin, int& end) {
+  const long long ntiles = (long long)p.N * p.th * p.tw * p.D;
+  begin = (int)(ntiles * blockIdx.x / gridDim.x);
+  end = (int)(ntiles * (blockIdx.x + 1) / gridDim.x);
 }
-constexpr int kHaloDepth = 6;          // cp.async groups (slices) in flight per loader thread; must be < ring slices
+
+// one column segment of a CTA's output range: nd output slices from (n, d0) of the (h0, w0) column
+struct Halo3Seg {
+  int n, h0, w0, d0, nd;
+};
+// the segment starting at output slice tile t of a CTA range that ends at `end` (tiles ordered (n, h tile, w tile, d))
+__device__ __forceinline__ Halo3Seg halo3_segment(const HaloArgs& p, int t, int end) {
+  Halo3Seg s;
+  s.d0 = t % p.D;
+  int c = t / p.D;
+  const int iw = c % p.tw;
+  c /= p.tw;
+  const int ih = c % p.th;
+  s.n = c / p.th;
+  s.w0 = iw * HT_W;
+  s.h0 = ih * HT_H;
+  s.nd = min(p.D - s.d0, end - t);
+  return s;
+}
 
 template <int CIN, int COUT, bool BWD>
 __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArgs p) {
@@ -387,7 +393,6 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
   constexpr uint32_t SLICE = (uint32_t)CP * PLANE;
   constexpr int taps = 27;
   constexpr uint32_t W_BYTES = (uint32_t)taps * CIN * COUT * 2u;
-  constexpr int R = kAccRing;
   uint8_t* s_w = smem;
   uint8_t* s_ring = smem + ((W_BYTES + 127u) & ~127u);
   uint8_t* tail = s_ring + (size_t)p.nslices * SLICE;
@@ -395,22 +400,18 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
   uint64_t* sfull = reinterpret_cast<uint64_t*>(tail);
   uint64_t* sempty = sfull + kHaloMaxSlices;
   uint64_t* tfull = sempty + kHaloMaxSlices;
-  uint64_t* tempty = tfull + R;
-  float* s_stat = reinterpret_cast<float*>(tempty + R);      // [4 epilogue warps][2][Cout]
+  uint64_t* tempty = tfull + 2;
+  float* s_stat = reinterpret_cast<float*>(tempty + 2);      // [4 epilogue warps][2][Cout]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
-  const int items_per_cta = (p.nitems + gridDim.x - 1) / gridDim.x;
-  const int item_begin = blockIdx.x * items_per_cta;
-  const int item_end = min(p.nitems, item_begin + items_per_cta);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nslices; ++s) {
       mbar_init(&sfull[s], 1);                   // ONE arrive: by the loader warp that staged the slice
       mbar_init(&sempty[s], 4);                  // one arrive per MMA warp
     }
-    for (int a = 0; a < R; ++a) {
+    for (int a = 0; a < 2; ++a) {
       mbar_init(&tfull[a], 4);
       mbar_init(&tempty[a], 4);
     }
@@ -420,9 +421,8 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
   float* s_bias = s_stat + 8 * COUT;
   float* s_ab = s_bias + COUT;                                       // [2][Cout]: A, B of the sample being processed
   double* s_gd = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(s_ab + 2 * COUT) + 7) & ~(uintptr_t)7);   // [2][Cout] + [8][2]
+  // staging tile [128 rows][2 buffers x Cout] fp32: completed outputs on their way from the MMA warpgroup to the epilogue
   float* s_acc = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(s_gd + 2 * COUT + 16) + 15) & ~(uintptr_t)15);
-  // the accumulator ring starts at zero (every MMA accumulates)
-  for (int i = threadIdx.x; i < 128 * p.acc_pitch; i += blockDim.x) s_acc[i] = 0.f;
   __syncthreads();
   // everything above is on-chip set-up and runs under the tail of the previous kernel; global memory from here on
   PDL_WAIT();
@@ -441,92 +441,102 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
   __syncthreads();
   constexpr int pd = 1;
 
-  auto decode = [&](int item, int& n, int& h0, int& w0, int& d0, int& nd) {
-    int t = item;
-    const int dc = t % p.ndchunks; t /= p.ndchunks;
-    const int iw = t % p.tw; t /= p.tw;
-    const int ih = t % p.th;
-    n = t / p.th;
-    w0 = iw * HT_W;
-    h0 = ih * HT_H;
-    d0 = dc * p.dchunk;
-    nd = min(p.dchunk, p.D - d0);
-  };
-
   if (warp < 4) {
     // ===================================================== MMA warpgroup
+    setmaxnreg_inc<kH3RegsMma>();
     const int wt = threadIdx.x;
     const uint64_t a_hi = make_nosw_desc(0, PLANE, HP_W * 16u);
-    const uint64_t b_hi = make_nosw_desc(0, 3u * COUT * 16u, 128u);
+    const uint64_t b_base = make_nosw_desc(smem_u32(s_w), 3u * COUT * 16u, 128u);
     const uint32_t ring_u32 = smem_u32(s_ring);
-    const uint32_t w_u32 = smem_u32(s_w);
-    uint32_t gs = 0;   // input slices consumed so far (ring position of the item's first slice)
-    uint32_t go = 0;   // output slices started so far (accumulator slot of the item's first output)
-    for (int item = item_begin; item < item_end; ++item) {
-      int n, h0, w0, d0, nd;
-      decode(item, n, h0, w0, d0, nd);
-      const int nsl = nd + KD - 1;
+    constexpr int kchunks = CIN / 16;
+    constexpr int F = COUT / 2;   // fragment registers of one output (Cout columns) per M64 half
+    // [M64 half][3 outputs x F]: while slice i is multiplied in, columns [0, F) hold output i-2, [F, 2F) output i-1
+    // and [2F, 3F) output i
+    float acc0[3 * F], acc1[3 * F];
+    frag_zero(acc0);
+    frag_zero(acc1);
+    int t_begin, t_end;
+    halo3_range(p, t_begin, t_end);
+    uint32_t gs = 0;   // input slices of earlier segments (ring position of the segment's first slice)
+    uint32_t go = 0;   // outputs of earlier segments (staging position of the segment's first output)
+    for (int t = t_begin; t < t_end;) {
+      const Halo3Seg s = halo3_segment(p, t, t_end);
+      const int nsl = s.nd + KD - 1;
       for (int i = 0; i < nsl; ++i) {
+        // [i-3, i-2, i-1] -> [i-2, i-1, i (zero)]
+#pragma unroll
+        for (int j = 0; j < 2 * F; ++j) {
+          acc0[j] = acc0[j + F];
+          acc1[j] = acc1[j + F];
+        }
+#pragma unroll
+        for (int j = 2 * F; j < 3 * F; ++j) acc0[j] = acc1[j] = 0.f;
         const uint32_t sl = gs + (uint32_t)i;
         mbar_wait(&sfull[sl % p.nslices], (sl / p.nslices) & 1u);
-        if (i < nd) {
-          // output i is touched for the first time: its slot must have been drained (and zeroed) by the epilogue
-          const uint32_t gn_ = go + (uint32_t)i;
-          mbar_wait(&tempty[gn_ % R], ((gn_ / R) & 1u) ^ 1u);
-        }
         // (the loader warp that staged the slice has waited for its cp.async group and executed
         //  fence.proxy.async BEFORE the arrive: the data is already ordered for the tensor core's async-proxy reads)
-        {
-          const int lo = i - 2 > 0 ? i - 2 : 0;
-          const int hi = i < nd - 1 ? i : nd - 1;
-          const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % p.nslices) * SLICE) >> 4);
-          // pieces of [lo, hi] that are contiguous in the accumulator ring
-          int o0 = lo;
-          while (o0 <= hi) {
-            const uint32_t slot0 = (go + (uint32_t)o0) % R;
-            int cnt = hi - o0 + 1;
-            if ((int)slot0 + cnt > R) cnt = R - (int)slot0;
-            float* acc = s_acc + slot0 * COUT;
-            const uint32_t row0 = (uint32_t)(2 - i + o0) * COUT;            // weight rows: kd = i - o  ->  (2 - kd) * Cout
-            const uint64_t b_base = b_hi | (uint64_t)((w_u32 + row0 * 16u) >> 4);
-            if (cnt == 1) halo3_mma<CIN, COUT, COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-            else if (cnt == 2) halo3_mma<CIN, COUT, 2 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-            else halo3_mma<CIN, COUT, 3 * COUT>(acc, p.acc_pitch, a_base, b_base, wt);
-            o0 += cnt;
+        const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % p.nslices) * SLICE) >> 4);
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        wgmma_fence();
+        // straight-line issue: every descriptor is (slice / weight base) + compile-time offset, in 16-byte units
+#pragma unroll
+        for (int t9 = 0; t9 < 9; ++t9)
+#pragma unroll
+          for (int kc = 0; kc < kchunks; ++kc) {
+            const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)((t9 / 3) * HP_W + (t9 % 3)) * 16u) >> 4;
+            const uint32_t b_off = ((uint32_t)(t9 * CP + 2 * kc) * 3u * COUT * 16u) >> 4;
+            Wgmma<3 * COUT, 0, 0>::mma(acc0, a_base + a_off, b_base + b_off);
+            Wgmma<3 * COUT, 0, 0>::mma(acc1, a_base + a_off + (8u * HP_W * 16u >> 4), b_base + b_off);   // hh 8..15
           }
+        wgmma_commit();
+        wgmma_wait0();
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sempty[sl % p.nslices]);   // this input slice is consumed
+        if (i >= 2) {
+          // output i-2 has all three contributions
+          const uint32_t o = go + (uint32_t)(i - 2);
+          const uint32_t as = o & 1u;
+          mbar_wait(&tempty[as], ((o >> 1) & 1u) ^ 1u);
+          frag_store(s_acc + as * COUT, p.acc_pitch, 0, reinterpret_cast<const float(&)[F]>(acc0[0]), wt);
+          frag_store(s_acc + as * COUT, p.acc_pitch, 64, reinterpret_cast<const float(&)[F]>(acc1[0]), wt);
           __syncwarp();
-          if (lane == 0) {
-            if (i >= 2) mbar_arrive(&tfull[(go + (uint32_t)(i - 2)) % R]);   // output i-2 has all three contributions
-            mbar_arrive(&sempty[sl % p.nslices]);                            // this input slice is consumed
-          }
+          if (lane == 0) mbar_arrive(&tfull[as]);
         }
       }
       gs += (uint32_t)nsl;
-      go += (uint32_t)nd;
+      go += (uint32_t)s.nd;
+      t += s.nd;
     }
   } else if (warp >= 8) {
     // ===================================================== loaders: 4 warps, warp w stages the input slices
     // sl = w (mod 4) on its own (all pieces of the slice, 16-byte cp.async with zero fill = conv padding), waits
     // for them to land and signals the slice with ONE mbarrier arrive.  The warps run independently: four slices
     // are in flight per CTA.
+    setmaxnreg_dec<kH3RegsLoad>();
     const int lw = warp - 8;
     constexpr int pieces = HP_H * HP_W * CP;
-    int it_item = item_begin, it_i = 0, it_nsl = 0, n = 0, h0 = 0, w0 = 0, d0 = 0, nd = 0;
-    auto load_item = [&]() {
-      if (it_item < item_end) {
-        decode(it_item, n, h0, w0, d0, nd);
-        it_nsl = nd + KD - 1;
+    int t_begin, t_end;
+    halo3_range(p, t_begin, t_end);
+    int t = t_begin, it_i = 0, it_nsl = 0;
+    Halo3Seg s{0, 0, 0, 0, 0};
+    auto load_seg = [&]() {
+      if (t < t_end) {
+        s = halo3_segment(p, t, t_end);
+        it_nsl = s.nd + KD - 1;
       }
     };
     auto advance = [&](int steps) {
       it_i += steps;
-      while (it_item < item_end && it_i >= it_nsl) {
+      while (t < t_end && it_i >= it_nsl) {
         it_i -= it_nsl;
-        ++it_item;
-        load_item();
+        t += s.nd;
+        load_seg();
       }
     };
-    load_item();
+    load_seg();
     advance(lw);
     uint32_t sl = (uint32_t)lw, prev_sl = 0u;
     bool have_prev = false;
@@ -535,18 +545,18 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
       __syncwarp();
       if (lane == 0) mbar_arrive(&sfull[which % p.nslices]);
     };
-    while (it_item < item_end) {
+    while (t < t_end) {
       const uint32_t slot = sl % p.nslices;
       mbar_wait(&sempty[slot], ((sl / p.nslices) & 1u) ^ 1u);
       const uint32_t dst = smem_u32(s_ring + (size_t)slot * SLICE);
-      const int d = d0 - pd + it_i;
+      const int d = s.d0 - pd + it_i;
       const bool dok = (unsigned)d < (unsigned)p.D;
-      const bf16* src = p.x + (((long long)n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
+      const bf16* src = p.x + (((long long)s.n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
 #pragma unroll 4
       for (int q = lane; q < pieces; q += 32) {
         const int v = q / CP, plane = q - v * CP;
         const int hh = v / HP_W, ww = v - hh * HP_W;
-        const int h = h0 - 1 + hh, w = w0 - 1 + ww;
+        const int h = s.h0 - 1 + hh, w = s.w0 - 1 + ww;
         const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
         const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
@@ -570,9 +580,10 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
     }
   } else {
     // ===================================================== epilogue warps 4..7
-    // GroupNorm statistics: per-thread (= per output row) partial sums in registers over ALL slices of an item, one
-    // butterfly fold over the warp per item (not per slice); bias from shared memory; the accumulator columns are
-    // zeroed right after the read and the slot is released before the arithmetic.
+    // GroupNorm statistics: per-thread (= per output row) partial sums in registers over ALL slices of a segment, one
+    // butterfly fold over the warp per segment (not per slice); bias from shared memory; the staging buffer is
+    // released right after the read, before the arithmetic.
+    setmaxnreg_inc<kH3RegsEpi>();
     const int q = warp & 3;
     const int row = q * 32 + lane;
     const int rw = row % HT_W, rh = row / HT_W;
@@ -631,9 +642,13 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
       asm volatile("bar.sync 1, 128;" ::: "memory");
     };
     const bool want_stats = p.stats != nullptr;
-    for (int item = item_begin; item < item_end; ++item) {
-      int n, h0, w0, d0, nd;
-      decode(item, n, h0, w0, d0, nd);
+    int t_begin, t_end;
+    halo3_range(p, t_begin, t_end);
+    for (int t = t_begin; t < t_end;) {
+      const Halo3Seg sg = halo3_segment(p, t, t_end);
+      const int n = sg.n, h0 = sg.h0, w0 = sg.w0, d0 = sg.d0, nd = sg.nd;
+      t += nd;
+      // a CTA's range can cross into the next sample: its statistics go to that sample's rows from here on
       if (n != cur_n) {
         if (cur_n >= 0 && want_stats) flush_stats(cur_n);
         cur_n = n;
@@ -666,18 +681,15 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
               yfv[k_] = *reinterpret_cast<const uint4*>(p.yfwd + vox * p.yfld + 8 * k_);
           }
         }
-        const uint32_t as = go % R;
-        mbar_wait(&tfull[as], (go / R) & 1u);
-        float* tacc = s_acc + row * p.acc_pitch + as * COUT;
+        const uint32_t as = go & 1u;
+        mbar_wait(&tfull[as], (go >> 1) & 1u);
+        const float* tacc = s_acc + row * p.acc_pitch + as * COUT;
 #pragma unroll
         for (int c0 = 0; c0 < COUT; c0 += 16) {
           float v[16];
           acc_ld16(tacc + c0, v);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)   // hand the columns back zeroed (all MMAs accumulate)
-            reinterpret_cast<float4*>(tacc + c0)[j] = make_float4(0.f, 0.f, 0.f, 0.f);
           if (c0 + 16 >= COUT) {
-            // every column of the slot is read and zeroed: release it before the arithmetic
+            // every column of the buffer is read: release it before the arithmetic
             __syncwarp();
             if (lane == 0) mbar_arrive(&tempty[as]);
           }
@@ -864,36 +876,41 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   p.th = (p.H + HT_H - 1) / HT_H;
   const int cols = p.N * p.th * p.tw;
   const int sms = num_sms(device);
-  // split d so that the grid covers the chip (each extra chunk re-loads kd-1 halo slices); one CTA per SM with a
-  // deep slice ring
+  // one CTA per SM with a deep slice ring; the 2-D kernel splits d so that the grid covers the chip
   const uint32_t slice = (uint32_t)(p.Cin / 8) * HP_H * HP_W * 16u;
   const uint32_t wbytes = ((uint32_t)(p.kd * 9) * p.Cin * p.Cout * 2u + 127u) & ~127u;
   uint32_t tail;
+  p.acc_pitch = 2 * p.Cout + 4;
   if (p.kd == 3) {
-    p.acc_pitch = kAccRing * p.Cout + 4;
-    tail = (2 * kHaloMaxSlices + 2 * kAccRing) * 8 + 16 + 11 * p.Cout * 4 + 64 + (2 * p.Cout + 16) * 8 + 8 + 16 +
+    tail = (2 * kHaloMaxSlices + 4) * 8 + 16 + 11 * p.Cout * 4 + 64 + (2 * p.Cout + 16) * 8 + 8 + 16 +
            128u * (uint32_t)p.acc_pitch * 4u;
   } else {
-    p.acc_pitch = 2 * p.Cout + 4;
     tail = (2 * kHaloMaxSlices + 4) * 8 + 16 + 8 * p.Cout * 4 + 64 + 16 + 128u * (uint32_t)p.acc_pitch * 4u;
   }
   const int slots = sms;
-  int ndch = 1;
-  if (cols < slots) {
-    ndch = slots / cols;               // items <= slots: one item per CTA, no second wave
-    if (ndch > p.D) ndch = p.D;
-    if (ndch < 1) ndch = 1;
+  int grid;
+  if (p.kd == 3) {
+    // the 3-D kernel splits the N * th * tw * D output slice tiles evenly over the CTAs
+    const long long ntiles = (long long)cols * p.D;
+    grid = ntiles < slots ? (int)ntiles : slots;
+  } else {
+    int ndch = 1;
+    if (cols < slots) {
+      ndch = slots / cols;               // items <= slots: one item per CTA, no second wave
+      if (ndch > p.D) ndch = p.D;
+      if (ndch < 1) ndch = 1;
+    }
+    p.dchunk = (p.D + ndch - 1) / ndch;
+    p.ndchunks = (p.D + p.dchunk - 1) / p.dchunk;
+    p.nitems = cols * p.ndchunks;
+    grid = slots < p.nitems ? slots : p.nitems;
   }
-  p.dchunk = (p.D + ndch - 1) / ndch;
-  p.ndchunks = (p.D + p.dchunk - 1) / p.dchunk;
-  p.nitems = cols * p.ndchunks;
   const int budget = maxsm;
   int ns = (int)((budget - 256 - (int)wbytes - (int)tail) / (int)slice);
   if (ns > kHaloMaxSlices) ns = kHaloMaxSlices;
   B200_CHECK_ARG(ns >= p.kd + 1, "conv_halo: slices do not fit in shared memory");
   p.nslices = ns;
   const size_t smem_bytes = 128 + wbytes + (size_t)ns * slice + tail;
-  int grid = slots < p.nitems ? slots : p.nitems;
 #define HALO_LAUNCH(CI, CO) launch_k(conv_halo_kernel<CI, CO>, grid, kHaloThreads, smem_bytes, st, p)
 #define HALO3_LAUNCH(CI, CO)                                                                             \
   do {                                                                                                   \
