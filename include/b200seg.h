@@ -52,6 +52,12 @@ extern "C" {
 #define B200SEG_LOSS_DICE 1
 #define B200SEG_LOSS_CE 2
 #define B200SEG_LOSS_FOCAL 4
+/* one of these alone (not combined with each other or with the three above) */
+#define B200SEG_LOSS_JACCARD 8    /* BinaryJaccardLoss, model/losses.py:19-30 */
+#define B200SEG_LOSS_ELDICE 16    /* BinaryELDiceLoss (C == 1) losses.py:66-74, MutilELDiceLoss (C > 1) :358-382 */
+#define B200SEG_LOSS_TVERSKY 32   /* BinaryTverskyLoss, losses.py:113-126 */
+#define B200SEG_LOSS_SS 64        /* BinarySSLoss, losses.py:87-99 (partials: b200seg_loss_partials_ss) */
+#define B200SEG_LOSS_EXT_MASK (B200SEG_LOSS_JACCARD | B200SEG_LOSS_ELDICE | B200SEG_LOSS_TVERSKY | B200SEG_LOSS_SS)
 
 typedef struct b200seg_tensor {
   void* ptr;       /* device pointer to element (0,0,0,0,0) */
@@ -225,11 +231,47 @@ int b200seg_head_probs(const float* logits, float* probs, int64_t nvox, int C, i
 int b200seg_loss_partials(const float* logits, const void* labels, int label_dtype, int N, int64_t vox_per_sample,
                           int C, float gamma, float alpha_f, double* part, double* metric, int device,
                           b200seg_stream stream);
-/* lcoef (fp32): C>1: a_c[C], b_c[C], ce_scale, focal_scale, gamma ; C==1: a, b, bce_scale, focal_scale, gamma */
+/* lcoef (fp32): C>1: a_c[C], b_c[C], ce_scale, focal_scale, gamma ; C==1: a, b, bce_scale, focal_scale, gamma
+ * terms JACCARD / ELDICE / TVERSKY (losses.py:19-30,66-74,113-126,358-382) write the same layout (a, b only), so
+ * b200seg_loss_bwd takes their gradient; TVERSKY reads alpha from alpha_f and beta from gamma.  SS (losses.py:87-99)
+ * reads r from alpha_f and the sums of b200seg_loss_partials_ss, writes lcoef = {r/(s+T), (1-r)/(s+V-T), 0, 0, 0}
+ * for b200seg_loss_bwd_ss. */
 int b200seg_loss_finalize(const double* part, int C, int terms, const float* alpha, float gamma, float alpha_f,
                           float* loss, float* lcoef, int device, b200seg_stream stream);
 int b200seg_loss_bwd(const float* logits, const void* labels, int label_dtype, int64_t nvox, int C,
                      const float* lcoef, const float* gscale, float* dlogits, int device, b200seg_stream stream);
+/* BinarySSLoss (losses.py:87-99), C == 1: part (double [7], += ) = {I, P, T, sum (p-t)^2 t, sum (p-t)^2 (1-t), V, 0};
+ * metric as b200seg_loss_partials.  Backward: dlogits = gscale 2 (p-t) (lcoef[0] t + lcoef[1] (1-t)) p (1-p). */
+int b200seg_loss_partials_ss(const float* logits, const void* labels, int label_dtype, int N, int64_t vox_per_sample,
+                             double* part, double* metric, int device, b200seg_stream stream);
+int b200seg_loss_bwd_ss(const float* logits, const void* labels, int label_dtype, int64_t nvox, const float* lcoef,
+                        const float* gscale, float* dlogits, int device, b200seg_stream stream);
+
+/* ---- stable segmented LSD radix sort of (uint32 key, int32 value) pairs, ascending by key, ties in input order:
+ * nseg segments of seg_len pairs each, segment s at [s*seg_len, (s+1)*seg_len).  Inputs are not modified;
+ * `workspace` of b200seg_radix_sort_workspace(nseg, seg_len) bytes.  seg_len < 2^31. */
+int64_t b200seg_radix_sort_workspace(int nseg, int64_t seg_len);
+int b200seg_radix_sort_pairs(const uint32_t* keys_in, const int32_t* vals_in, uint32_t* keys_out, int32_t* vals_out,
+                             int nseg, int64_t seg_len, void* workspace, int64_t workspace_bytes, int device,
+                             b200seg_stream stream);
+
+/* ---- Lovasz-Softmax (LovaszLoss, model/losses.py:462-473 -> model/lovasz.py:90-138), C >= 2.  The logits are the
+ * "probabilities", as LovaszLoss.forward passes them (lovasz.py:133).  Per class c over the flattened P = n*vox + v
+ * (lovasz.py:141-158; per_image: per sample n), skipping voxels labelled `ignore` (if has_ignore): e = |[t==c] - z_c|
+ * sorted descending (stable: ties in ascending P), grad = Lovasz gradient of the sorted [t==c] (lovasz.py:21-32);
+ * class loss = dot(e_sorted, grad); classes with no voxel of the class are skipped (lovasz.py:125); loss = mean over
+ * the rest (0 if none; per_image: the mean over samples of those means).  Labels outside [0, C) are background for
+ * every class.  logits fp32 channels-last [N][vox][C], labels int64 [N][vox].
+ * b200seg_lovasz_fwd writes loss, coef [N][vox][C] (the Lovasz gradient of every voxel and class, 0 where ignored)
+ * and seg_scale [S] (S = C, or N*C with per_image: the weight of each class segment in the mean).
+ * b200seg_lovasz_bwd: dlogits = gscale * coef * sgn(z_c - [t==c]) * seg_scale.  Segments must hold < 2^31 voxels. */
+int64_t b200seg_lovasz_workspace(int N, int64_t vox_per_sample, int C, int per_image);
+int b200seg_lovasz_fwd(const float* logits, const int64_t* labels, int N, int64_t vox_per_sample, int C, int per_image,
+                       int has_ignore, int64_t ignore, void* workspace, int64_t workspace_bytes, float* loss,
+                       float* coef, float* seg_scale, int device, b200seg_stream stream);
+int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_t vox_per_sample, int C, int per_image,
+                       const float* coef, const float* seg_scale, const float* gscale, float* dlogits, int device,
+                       b200seg_stream stream);
 
 /* ---- per-step accuracy (model/metric.py:146-181).  b200seg_metric_partials: the sums above from MATERIALISED
  * probabilities (fp32 channels-last [N][vox][C], threshold 0.5 in the reference); b200seg_metric_finalize:

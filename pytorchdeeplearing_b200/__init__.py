@@ -1,7 +1,7 @@
 """pytorchdeeplearing_b200 -- H100-native (sm_90a) drop-in for the segmentation hot path of
 junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
-``networks/Unet2d.py`` forward/backward and the Dice / BCE / focal / CE reductions of
-``model/losses.py`` (SURVEY.md section 8).
+``networks/Unet2d.py`` forward/backward and the losses of ``model/losses.py`` (Dice / BCE / focal / CE,
+Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -13,7 +13,8 @@ from .runtime import (set_precision, get_precision, enable_data_parallel, disabl
 from .networks import VNet3d, VNet2d, UNet3d, UNet2d, initialize_weights
 from .losses import (BinaryDiceLoss, BinaryCrossEntropyLoss, BinaryFocalLoss, BinaryCrossEntropyDiceLoss,
                      BinaryDiceFocalLoss, MutilCrossEntropyLoss, MutilFocalLoss, MutilDiceLoss,
-                     MutilCrossEntropyDiceLoss)
+                     MutilCrossEntropyDiceLoss, BinaryJaccardLoss, BinaryELDiceLoss, BinarySSLoss, BinaryTverskyLoss,
+                     MutilELDiceLoss, LovaszLoss)
 from .install import install, uninstall
 from .graphed import GraphedStep
 from .optim import FusedAdamW, FusedAdam
@@ -27,4 +28,5 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "initialize_weights", "FusedA
            "enable_data_parallel", "disable_data_parallel", "install", "uninstall", "GraphedStep",
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
-           "MutilCrossEntropyDiceLoss"]
+           "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
+           "MutilELDiceLoss", "LovaszLoss"]

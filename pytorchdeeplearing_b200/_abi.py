@@ -81,6 +81,13 @@ _SIGNATURES = {
     "b200seg_loss_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _f, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_loss_finalize": ([_vp, _i, _i, _vp, _f, _f, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_loss_bwd": ([_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_loss_partials_ss": ([_vp, _vp, _i, _i, _i64, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_loss_bwd_ss": ([_vp, _vp, _i, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_radix_sort_workspace": ([_i, _i64], C.c_int64),
+    "b200seg_radix_sort_pairs": ([_vp, _vp, _vp, _vp, _i, _i64, _vp, _i64, _i, _vp], C.c_int),
+    "b200seg_lovasz_workspace": ([_i, _i64, _i, _i], C.c_int64),
+    "b200seg_lovasz_fwd": ([_vp, _vp, _i, _i64, _i, _i, _i, _i64, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_lovasz_bwd": ([_vp, _vp, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_metric_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _vp, _i, _vp], C.c_int),
     "b200seg_metric_finalize": ([_vp, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _i, _i, _vp], C.c_int),
@@ -529,6 +536,53 @@ class CudaBackend:
         self._check(self.lib.b200seg_loss_bwd(logits.data_ptr(), labels.data_ptr(), self._label_dtype(labels),
                                               logits.numel() // c, c, lcoef.data_ptr(), gscale.data_ptr(),
                                               dlogits.data_ptr(), dev, st))
+
+    def loss_partials_ss(self, logits, labels, part, metric=None):
+        """BinarySSLoss sums (include/b200seg.h: b200seg_loss_partials_ss), same part size as the binary losses"""
+        dev, st = self._ds(logits)
+        n = logits.shape[0]
+        self._check(self.lib.b200seg_loss_partials_ss(logits.data_ptr(), labels.data_ptr(), self._label_dtype(labels),
+                                                      n, logits.numel() // n, part.data_ptr(), _p(metric), dev, st))
+
+    def loss_bwd_ss(self, logits, labels, lcoef, gscale, dlogits):
+        dev, st = self._ds(logits)
+        self._check(self.lib.b200seg_loss_bwd_ss(logits.data_ptr(), labels.data_ptr(), self._label_dtype(labels),
+                                                 logits.numel(), lcoef.data_ptr(), gscale.data_ptr(),
+                                                 dlogits.data_ptr(), dev, st))
+
+    def radix_sort_pairs(self, keys, vals):
+        """keys uint32 bit patterns in int32 [nseg, len], vals int32 [nseg, len] -> (keys, vals) sorted per row,
+        ascending by unsigned key, ties in input order"""
+        dev, st = self._ds(keys)
+        assert keys.dtype == torch.int32 and vals.dtype == torch.int32 and keys.shape == vals.shape and keys.dim() == 2
+        keys, vals = keys.contiguous(), vals.contiguous()
+        nseg, ln = keys.shape
+        ko, vo = torch.empty_like(keys), torch.empty_like(vals)
+        nb = int(self.lib.b200seg_radix_sort_workspace(nseg, ln))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=keys.device)
+        self._check(self.lib.b200seg_radix_sort_pairs(keys.data_ptr(), vals.data_ptr(), ko.data_ptr(), vo.data_ptr(),
+                                                      nseg, ln, ws.data_ptr(), nb, dev, st))
+        return ko, vo
+
+    def lovasz_fwd(self, logits, labels, per_image, ignore, loss, coef, seg_scale):
+        """logits (N, ..., C) fp32 channels-last contiguous, labels int64 (N, ...); coef like logits;
+        seg_scale fp32 [N*C if per_image else C].  ignore: None or an int label value"""
+        dev, st = self._ds(logits)
+        n, c = logits.shape[0], logits.shape[-1]
+        vox = logits.numel() // (n * c)
+        nb = int(self.lib.b200seg_lovasz_workspace(n, vox, c, 1 if per_image else 0))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=logits.device)
+        self._check(self.lib.b200seg_lovasz_fwd(logits.data_ptr(), labels.data_ptr(), n, vox, c,
+                                                1 if per_image else 0, 0 if ignore is None else 1,
+                                                0 if ignore is None else int(ignore), ws.data_ptr(), nb,
+                                                loss.data_ptr(), coef.data_ptr(), seg_scale.data_ptr(), dev, st))
+
+    def lovasz_bwd(self, logits, labels, per_image, coef, seg_scale, gscale, dlogits):
+        dev, st = self._ds(logits)
+        n, c = logits.shape[0], logits.shape[-1]
+        self._check(self.lib.b200seg_lovasz_bwd(logits.data_ptr(), labels.data_ptr(), n, logits.numel() // (n * c), c,
+                                                1 if per_image else 0, coef.data_ptr(), seg_scale.data_ptr(),
+                                                gscale.data_ptr(), dlogits.data_ptr(), dev, st))
 
     # ------------------------------------------------------------------ per-step accuracy (model/metric.py)
     def metric_partials(self, probs, labels, threshold, metric):

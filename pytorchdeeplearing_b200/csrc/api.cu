@@ -121,6 +121,19 @@ int loss_finalize(const double* part, int C, int terms, const float* alpha, floa
                   float* lcoef, cudaStream_t s);
 int loss_bwd(const float* logits, const void* labels, int label_dtype, long long nvox_, int C, const float* lcoef,
              const float* gscale, float* dlogits, int device, cudaStream_t s);
+int loss_partials_ss(const float* logits, const void* labels, int label_dtype, int N, long long vox, double* part,
+                     double* metric, int device, cudaStream_t s);
+int loss_bwd_ss(const float* logits, const void* labels, int label_dtype, long long nvox_, const float* lcoef,
+                const float* gscale, float* dlogits, int device, cudaStream_t s);
+int64_t radix_sort_workspace(int nseg, long long len);
+int radix_sort_pairs(const uint32_t* kin, const int32_t* vin, uint32_t* kout, int32_t* vout, int nseg, long long len,
+                     void* ws, long long ws_bytes, cudaStream_t s);
+int64_t lovasz_workspace(int N, long long vox, int C, int per_image);
+int lovasz_fwd(const float* z, const long long* t, int N, long long vox, int C, int per_image, int has_ignore,
+               long long ignore, void* ws, long long ws_bytes, float* loss, float* coef, float* seg_scale, int device,
+               cudaStream_t s);
+int lovasz_bwd(const float* z, const long long* t, int N, long long vox, int C, int per_image, const float* coef,
+               const float* seg_scale, const float* gscale, float* dz, int device, cudaStream_t s);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -518,7 +531,10 @@ int b200seg_stage_labels_u8(const uint8_t* lab, int64_t count, int binarize, int
 int b200seg_loss_finalize(const double* part, int C, int terms, const float* alpha, float gamma, float alpha_f,
                           float* loss, float* lcoef, int device, b200seg_stream stream) {
   B200_CHECK_ARG(part && loss && lcoef && C >= 1 && (C == 1 || alpha), "b200seg_loss_finalize: bad argument");
-  B200_CHECK_ARG(terms > 0 && terms < 8, "b200seg_loss_finalize: bad terms mask %d", terms);
+  const int ext = terms & B200SEG_LOSS_EXT_MASK;
+  B200_CHECK_ARG((terms > 0 && terms < 8) ||
+                     (terms == ext && (ext & (ext - 1)) == 0 && (C == 1 || ext == B200SEG_LOSS_ELDICE)),
+                 "b200seg_loss_finalize: bad terms mask %d for %d classes", terms, C);
   B200_DEVICE(device);
   return loss_finalize(part, C, terms, alpha, gamma, alpha_f, loss, lcoef, ST(stream));
 }
@@ -528,6 +544,58 @@ int b200seg_loss_bwd(const float* logits, const void* labels, int label_dtype, i
   B200_CHECK_ARG(logits && labels && lcoef && gscale && dlogits && nvox_ > 0, "b200seg_loss_bwd: bad argument");
   B200_DEVICE(device);
   return loss_bwd(logits, labels, label_dtype, nvox_, C, lcoef, gscale, dlogits, device, ST(stream));
+}
+
+int b200seg_loss_partials_ss(const float* logits, const void* labels, int label_dtype, int N, int64_t vox,
+                             double* part, double* metric, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(logits && labels && part && vox > 0 && N > 0, "b200seg_loss_partials_ss: bad argument");
+  B200_CHECK_ARG(label_dtype == B200SEG_I64 || label_dtype == B200SEG_F32, "b200seg_loss_partials_ss: bad label dtype");
+  B200_DEVICE(device);
+  return loss_partials_ss(logits, labels, label_dtype, N, vox, part, metric, device, ST(stream));
+}
+
+int b200seg_loss_bwd_ss(const float* logits, const void* labels, int label_dtype, int64_t nvox_, const float* lcoef,
+                        const float* gscale, float* dlogits, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(logits && labels && lcoef && gscale && dlogits && nvox_ > 0, "b200seg_loss_bwd_ss: bad argument");
+  B200_CHECK_ARG(label_dtype == B200SEG_I64 || label_dtype == B200SEG_F32, "b200seg_loss_bwd_ss: bad label dtype");
+  B200_DEVICE(device);
+  return loss_bwd_ss(logits, labels, label_dtype, nvox_, lcoef, gscale, dlogits, device, ST(stream));
+}
+
+int64_t b200seg_radix_sort_workspace(int nseg, int64_t seg_len) {
+  if (nseg < 1 || seg_len < 0) return 0;
+  return radix_sort_workspace(nseg, seg_len);
+}
+
+int b200seg_radix_sort_pairs(const uint32_t* keys_in, const int32_t* vals_in, uint32_t* keys_out, int32_t* vals_out,
+                             int nseg, int64_t seg_len, void* workspace, int64_t workspace_bytes, int device,
+                             b200seg_stream stream) {
+  B200_CHECK_ARG(seg_len == 0 || (keys_in && vals_in && keys_out && vals_out), "b200seg_radix_sort_pairs: null argument");
+  B200_DEVICE(device);
+  return radix_sort_pairs(keys_in, vals_in, keys_out, vals_out, nseg, seg_len, workspace, workspace_bytes, ST(stream));
+}
+
+int64_t b200seg_lovasz_workspace(int N, int64_t vox, int C, int per_image) {
+  if (N < 1 || vox < 1 || C < 1) return 0;
+  return lovasz_workspace(N, vox, C, per_image);
+}
+
+int b200seg_lovasz_fwd(const float* logits, const int64_t* labels, int N, int64_t vox, int C, int per_image,
+                       int has_ignore, int64_t ignore, void* workspace, int64_t workspace_bytes, float* loss,
+                       float* coef, float* seg_scale, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(logits && labels && loss && coef && seg_scale, "b200seg_lovasz_fwd: null argument");
+  B200_DEVICE(device);
+  return lovasz_fwd(logits, reinterpret_cast<const long long*>(labels), N, vox, C, per_image, has_ignore, ignore,
+                    workspace, workspace_bytes, loss, coef, seg_scale, device, ST(stream));
+}
+
+int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_t vox, int C, int per_image,
+                       const float* coef, const float* seg_scale, const float* gscale, float* dlogits, int device,
+                       b200seg_stream stream) {
+  B200_CHECK_ARG(logits && labels && coef && seg_scale && gscale && dlogits, "b200seg_lovasz_bwd: null argument");
+  B200_DEVICE(device);
+  return lovasz_bwd(logits, reinterpret_cast<const long long*>(labels), N, vox, C, per_image, coef, seg_scale, gscale,
+                    dlogits, device, ST(stream));
 }
 
 }  // extern "C"

@@ -460,6 +460,159 @@ __global__ void __launch_bounds__(256) loss_bwd_multi_generic_kernel(const float
   }
 }
 
+// ---- binary sensitivity-specificity (BinarySSLoss, model/losses.py:87-99): the binary sums with the two squared-error
+// sums in place of the cross-entropy ones.  part = {I, P, T, sum (p-t)^2 t, sum (p-t)^2 (1-t), V, 0}; metric as above
+template <typename TL>
+__global__ void __launch_bounds__(256) loss_partials_ss_kernel(const float* __restrict__ z, const TL* __restrict__ t,
+                                                               long long vox, double* __restrict__ part,
+                                                               double* __restrict__ metric) {
+  PDL_ENTER();
+  __shared__ double s_tmp[8];
+  const long long base = (long long)blockIdx.y * vox;
+  float aI = 0.f, aP = 0.f, aT = 0.f, aF = 0.f, aB = 0.f, mI = 0.f, mA = 0.f;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < vox;
+       i += (long long)gridDim.x * blockDim.x) {
+    const float zi = z[base + i];
+    const float ti = (float)t[base + i];
+    const float p = 1.f / (1.f + expf(-zi));
+    const float d = p - ti;
+    const float d2 = d * d;
+    aI = fmaf(p, ti, aI);
+    aP += p;
+    aT += ti;
+    aF = fmaf(d2, ti, aF);
+    aB = fmaf(d2, 1.f - ti, aB);
+    if (p > 0.5f) {
+      mI += ti;
+      mA += 1.f;
+    }
+  }
+  block_reduce_to_global((double)aI, part + 0, s_tmp);
+  block_reduce_to_global((double)aP, part + 1, s_tmp);
+  block_reduce_to_global((double)aT, part + 2, s_tmp);
+  block_reduce_to_global((double)aF, part + 3, s_tmp);
+  block_reduce_to_global((double)aB, part + 4, s_tmp);
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(part + 5, (double)vox);
+  if (metric != nullptr) {
+    double* m = metric + (long long)blockIdx.y * 3;
+    block_reduce_to_global((double)mI, m + 0, s_tmp);
+    block_reduce_to_global((double)mA, m + 1, s_tmp);
+    block_reduce_to_global((double)aT, m + 2, s_tmp);
+  }
+}
+
+// torch.clamp(x, 0, 2): the value, and whether the gradient passes (clamp backward keeps it for 0 <= x <= 2)
+__device__ __forceinline__ double clamp02(double x, bool* pass) {
+  *pass = x >= 0.0 && x <= 2.0;
+  return x < 0.0 ? 0.0 : (x > 2.0 ? 2.0 : x);
+}
+
+// ---- finalize of the Jaccard / exponential-log Dice / Tversky / sensitivity-specificity losses (one term bit each):
+// the value and the lcoef layout of loss_finalize_kernel, so loss_bwd_*_kernel serve all but SS unchanged.
+// TVERSKY: alpha_f = alpha, gamma = beta; SS: alpha_f = r.
+__global__ void loss_finalize_ext_kernel(const double* __restrict__ part, int C, int terms,
+                                         const float* __restrict__ alpha, float gamma, float alpha_f,
+                                         float* __restrict__ loss, float* __restrict__ lcoef) {
+  PDL_ENTER();
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  const double s = 1e-5, eps = 1e-7;
+  double val = 0.0;
+  if (C == 1) {
+    const double I = part[0], P = part[1], T = part[2];
+    double a = 0.0, b = 0.0;
+    bool pass = true;
+    if (terms == B200SEG_LOSS_JACCARD) {                  // losses.py:26-30: 1 - (I+s) / max(P+T-I+s, eps)
+      const double U = P + T - I + s;
+      if (U >= eps) {
+        val = 1.0 - (I + s) / U;
+        a = -1.0 / U - (I + s) / (U * U);
+        b = (I + s) / (U * U);
+      } else {
+        val = 1.0 - (I + s) / eps;
+        a = -1.0 / eps;
+      }
+    } else if (terms == B200SEG_LOSS_ELDICE) {            // losses.py:72-74: clamp((-log(dsc+s))^0.3, 0, 2)
+      const double D = P + T + s;
+      const double Dc = D < eps ? eps : D;
+      const double dsc = (2.0 * I + s) / Dc;
+      const double u = -log(dsc + s);
+      val = clamp02(pow(u, 0.3), &pass);
+      if (pass) {
+        const double k = -0.3 * pow(u, -0.7) / (dsc + s);      // d loss / d dsc
+        a = 2.0 * k / Dc;
+        b = D >= eps ? -k * (2.0 * I + s) / (D * D) : 0.0;
+      }
+    } else if (terms == B200SEG_LOSS_TVERSKY) {           // losses.py:120-126, fp = P-I, fn = T-I
+      const double al = alpha_f, be = gamma;
+      const double Dt = I + al * (P - I) + be * (T - I) + s;
+      val = clamp02(1.0 - (I + s) / Dt, &pass);
+      if (pass) {
+        a = -1.0 / Dt + (I + s) * (1.0 - al - be) / (Dt * Dt);
+        b = (I + s) * al / (Dt * Dt);
+      }
+    } else {                                              // SS, losses.py:94-99
+      const double Sf = part[3], Sb = part[4], V = part[5], r = alpha_f;
+      val = r * Sf / (s + T) + (1.0 - r) * Sb / (s + V - T);
+      a = r / (s + T);                                    // loss_bwd_ss_kernel: fg and bg weights
+      b = (1.0 - r) / (s + V - T);
+    }
+    lcoef[0] = (float)a;
+    lcoef[1] = (float)b;
+    lcoef[2] = 0.f;
+    lcoef[3] = 0.f;
+    lcoef[4] = 0.f;
+  } else {                                                // ELDICE, losses.py:372-382
+    const double* I = part;
+    const double* Ps = part + C;
+    const double* Cn = part + 2 * C;
+    double K = 0.0, S = 0.0;
+    for (int c = 0; c < C; ++c) {
+      K += Cn[c] > 0.0 ? 1.0 : 0.0;
+      const double draw = (2.0 * I[c] + s) / (Cn[c] + Ps[c] + s);
+      const double d = draw < eps ? eps : draw;
+      const double dice = Cn[c] > 0.0 ? d * (double)alpha[c] : 0.0;
+      S += pow(-log(dice + s), 0.3);                      // absent classes add (-log s)^0.3
+    }
+    bool pass;
+    val = clamp02(S / K, &pass);
+    for (int c = 0; c < C; ++c) {
+      double a = 0.0, b = 0.0;
+      const double D = Cn[c] + Ps[c];
+      const double draw = (2.0 * I[c] + s) / (D + s);
+      if (pass && Cn[c] > 0.0 && draw >= eps) {
+        const double al = alpha[c];
+        const double dice = draw * al;
+        const double k = -0.3 * pow(-log(dice + s), -0.7) / (dice + s) * al / K;    // d loss / d d_c
+        a = 2.0 * k / (D + s);
+        b = -k * (2.0 * I[c] + s) / ((D + s) * (D + s));
+      }
+      lcoef[c] = (float)a;
+      lcoef[C + c] = (float)b;
+    }
+    lcoef[2 * C] = 0.f;
+    lcoef[2 * C + 1] = 0.f;
+    lcoef[2 * C + 2] = 0.f;
+    if (part[3 * C + 3] > 0.0) val = __longlong_as_double(0x7ff8000000000000LL);   // labels outside [0, C)
+  }
+  loss[0] = (float)val;
+}
+
+// ---- BinarySSLoss backward: 2 (p-t) (r t / (s+T) + (1-r)(1-t) / (s+V-T)) p (1-p); lcoef[0..1] from the finalize
+template <typename TL>
+__global__ void __launch_bounds__(256) loss_bwd_ss_kernel(const float* __restrict__ z, const TL* __restrict__ t,
+                                                          long long nvox, const float* __restrict__ lcoef,
+                                                          const float* __restrict__ gscale, float* __restrict__ dz) {
+  PDL_ENTER();
+  const float wf = lcoef[0], wb = lcoef[1], gs = gscale[0];
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nvox;
+       i += (long long)gridDim.x * blockDim.x) {
+    const float ti = (float)t[i];
+    const float p = 1.f / (1.f + expf(-z[i]));
+    const float g = 2.f * (p - ti) * (wf * ti + wb * (1.f - ti)) * p * (1.f - p);
+    dz[i] = g * gs;
+  }
+}
+
 static int loss_blocks(long long nvox_, int device) {
   long long blocks = (nvox_ + 256 * 4 - 1) / (256 * 4);
   long long cap = (long long)num_sms(device) * 8;
@@ -532,7 +685,10 @@ int metric_finalize(const double* metric, int N, int C, float* out, cudaStream_t
 
 int loss_finalize(const double* part, int C, int terms, const float* alpha, float gamma, float alpha_f, float* loss,
                   float* lcoef, cudaStream_t s) {
-  launch_k(loss_finalize_kernel, 1, 32, 0, s, part, C, terms, alpha, gamma, alpha_f, loss, lcoef);
+  if (terms & B200SEG_LOSS_EXT_MASK)
+    launch_k(loss_finalize_ext_kernel, 1, 32, 0, s, part, C, terms, alpha, gamma, alpha_f, loss, lcoef);
+  else
+    launch_k(loss_finalize_kernel, 1, 32, 0, s, part, C, terms, alpha, gamma, alpha_f, loss, lcoef);
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }
@@ -562,6 +718,33 @@ int loss_bwd(const float* logits, const void* labels_, int label_dtype, long lon
     default:
       launch_k(loss_bwd_multi_generic_kernel, blocks, 256, 0, s, logits, labels, nvox_, C, lcoef, gscale, dlogits);
   }
+  B200_LAUNCH_CHECK();
+  return B200SEG_OK;
+}
+
+int loss_partials_ss(const float* logits, const void* labels, int label_dtype, int N, long long vox, double* part,
+                     double* metric, int device, cudaStream_t s) {
+  B200_CHECK_ARG(N >= 1 && N <= 65535, "loss_partials_ss: unsupported batch size %d", N);
+  const dim3 grid = sample_grid(vox, N, device);
+  if (label_dtype == B200SEG_F32)
+    launch_k(loss_partials_ss_kernel<float>, grid, 256, 0, s, logits, static_cast<const float*>(labels), vox, part,
+             metric);
+  else
+    launch_k(loss_partials_ss_kernel<long long>, grid, 256, 0, s, logits, static_cast<const long long*>(labels), vox,
+             part, metric);
+  B200_LAUNCH_CHECK();
+  return B200SEG_OK;
+}
+
+int loss_bwd_ss(const float* logits, const void* labels, int label_dtype, long long nvox_, const float* lcoef,
+                const float* gscale, float* dlogits, int device, cudaStream_t s) {
+  const int blocks = loss_blocks(nvox_, device);
+  if (label_dtype == B200SEG_F32)
+    launch_k(loss_bwd_ss_kernel<float>, blocks, 256, 0, s, logits, static_cast<const float*>(labels), nvox_, lcoef,
+             gscale, dlogits);
+  else
+    launch_k(loss_bwd_ss_kernel<long long>, blocks, 256, 0, s, logits, static_cast<const long long*>(labels), nvox_,
+             lcoef, gscale, dlogits);
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }

@@ -35,7 +35,7 @@ import torch
 
 from . import runtime
 from .engine import Engine
-from .losses import loss_spec, prepare_labels
+from .losses import LOVASZ, SS, ignore_label, loss_spec, lovasz_check, lovasz_scale_size, prepare_labels
 
 
 def _is_fused_optimizer(opt) -> bool:
@@ -60,6 +60,9 @@ class GraphedStep:
         self.use_graph = use_graph and x.is_cuda
         self.graphs = []             # [(graph, eager callable to run after it or None)]
         self._terms, self._alpha, self._gamma, self._alpha_f = loss_spec(lossfn)
+        if self._terms == LOVASZ:
+            lovasz_check(c)
+            self._per_image, self._ignore = bool(lossfn.per_image), ignore_label(lossfn.ignore)
         dev = self.x.device
         self._one = torch.ones(1, dtype=torch.float32, device=dev)
         # class weights of the loss: a constant of the step, created once (not a fill launch inside every step)
@@ -107,7 +110,10 @@ class GraphedStep:
         c, n = z.shape[-1], z.shape[0]
         buf = torch.zeros(be.part_size(c) + n * c * 3, dtype=torch.float64, device=z.device)
         part, metric = buf[:be.part_size(c)], buf[be.part_size(c):].view(n, c, 3)
-        be.loss_partials(z, self.y, self._gamma, self._alpha_f, part, metric)
+        if self._terms == SS:
+            be.loss_partials_ss(z, self.y, part, metric)
+        else:
+            be.loss_partials(z, self.y, self._gamma, self._alpha_f, part, metric)
         acc = torch.empty(2, dtype=torch.float32, device=z.device)
         be.metric_finalize(metric, acc)
         self._eng, self._z, self._part, self.probs, self._acc = eng, z, part, probs, acc
@@ -132,10 +138,19 @@ class GraphedStep:
         c = z.shape[-1]
         dev = z.device
         loss = torch.empty((), dtype=torch.float32, device=dev)
-        lcoef = torch.empty(2 * c + 3 if c > 1 else 5, dtype=torch.float32, device=dev)
-        be.loss_finalize(part, c, self._terms, self._alpha_t, self._gamma, self._alpha_f, loss, lcoef)
         dz = torch.empty_like(z)
-        be.loss_bwd(z, self.y, lcoef, self._one, dz)
+        if self._terms == LOVASZ:
+            coef = torch.empty_like(z)
+            scale = torch.empty(lovasz_scale_size(z.shape[0], c, self._per_image), dtype=torch.float32, device=dev)
+            be.lovasz_fwd(z, self.y, self._per_image, self._ignore, loss, coef, scale)
+            be.lovasz_bwd(z, self.y, self._per_image, coef, scale, self._one, dz)
+        else:
+            lcoef = torch.empty(2 * c + 3 if c > 1 else 5, dtype=torch.float32, device=dev)
+            be.loss_finalize(part, c, self._terms, self._alpha_t, self._gamma, self._alpha_f, loss, lcoef)
+            if self._terms == SS:
+                be.loss_bwd_ss(z, self.y, lcoef, self._one, dz)
+            else:
+                be.loss_bwd(z, self.y, lcoef, self._one, dz)
         g = dz if dz.dim() == 5 else dz.unsqueeze(1)
         self._split_off = None
         eng.bucket_hook = self._bucket_ready if self.dp else None
@@ -295,8 +310,8 @@ class GraphedStep:
     def check_labels(self) -> None:
         """Raise if the last step saw a label outside [0, numclass) (the reference raises in F.one_hot /
         F.cross_entropy; a captured step cannot, so the loss becomes NaN and this check names the cause).
-        Synchronises."""
-        if self.ncls > 1:
+        Synchronises.  LovaszLoss takes such labels as background (the reference does not raise there)."""
+        if self.ncls > 1 and self._terms != LOVASZ:
             bad = int(self._part[-1].item())
             if bad:
                 raise RuntimeError(f"{bad} label value(s) outside [0, {self.ncls})")

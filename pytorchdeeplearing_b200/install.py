@@ -16,6 +16,9 @@ _NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet2d")
 _METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff")
 _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
+# the further model/losses.py classes (bound there, not imported by the wrappers)
+_EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss", "MutilELDiceLoss",
+                   "LovaszLoss")
 _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet2d", "model",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet")
 
@@ -24,7 +27,7 @@ def install() -> int:
     """Rebind the reference's names to the drop-in implementations. Returns the number of bindings changed."""
     from . import networks as nets, losses, metric
     table = {n: getattr(nets, n) for n in _NET_NAMES}
-    table.update({n: getattr(losses, n) for n in _LOSS_NAMES})
+    table.update({n: getattr(losses, n) for n in _LOSS_NAMES + _EXT_LOSS_NAMES})
     table.update({n: getattr(metric, n) for n in _METRIC_NAMES})     # per-step accuracy, model/modelVNet.py:582
     count = 0
     for modname in _MODULES:

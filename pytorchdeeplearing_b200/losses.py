@@ -18,6 +18,8 @@ import torch.nn as nn
 from . import runtime
 
 DICE, CE, FOCAL = 1, 2, 4
+JACCARD, ELDICE, TVERSKY, SS = 8, 16, 32, 64     # include/b200seg.h B200SEG_LOSS_*: each one alone
+LOVASZ = 128                                     # not a finalize term: the sort-based Lovasz-Softmax path
 
 
 def _check_labels_default() -> bool:
@@ -63,7 +65,10 @@ class _FusedLoss(torch.autograd.Function):
         n = z.shape[0]
         buf = torch.zeros(be.part_size(c) + n * c * 3, dtype=torch.float64, device=dev)
         part, metric = buf[:be.part_size(c)], buf[be.part_size(c):].view(n, c, 3)
-        be.loss_partials(z, t, float(gamma), float(alpha_f), part, metric)
+        if terms == SS:
+            be.loss_partials_ss(z, t, part, metric)
+        else:
+            be.loss_partials(z, t, float(gamma), float(alpha_f), part, metric)
         enabled, group = runtime.dp_state()
         if enabled:
             import torch.distributed as dist
@@ -83,6 +88,7 @@ class _FusedLoss(torch.autograd.Function):
             owner._metric_sums = metric               # per-sample sums of the step's accuracy (SURVEY 8f-2)
         ctx.save_for_backward(z, t, lcoef)
         ctx.perm = perm
+        ctx.terms = terms
         return loss
 
     @staticmethod
@@ -91,9 +97,70 @@ class _FusedLoss(torch.autograd.Function):
         be = runtime.get_backend(z)
         dz = torch.empty_like(z)
         g = gout.detach().to(torch.float32).reshape(1).contiguous()
-        be.loss_bwd(z, t, lcoef, g, dz)
+        if ctx.terms == SS:
+            be.loss_bwd_ss(z, t, lcoef, g, dz)
+        else:
+            be.loss_bwd(z, t, lcoef, g, dz)
         inv = (0, 4, 1, 2, 3) if z.dim() == 5 else (0, 3, 1, 2)
         return dz.permute(*inv), None, None, None, None, None, None
+
+
+def ignore_label(ignore):
+    """the label value LovaszLoss(ignore=...) drops, as an int, or None (no integer label can equal it)"""
+    if ignore is None:
+        return None
+    v = float(ignore)
+    return int(v) if v.is_integer() else None
+
+
+def lovasz_check(c: int) -> None:
+    """what the reference raises for LovaszLoss on this class count / run mode"""
+    if c == 1:
+        # model/lovasz.py:127-129 with classes="present" (the only form LovaszLoss uses)
+        raise ValueError("Sigmoid output possible only with 1 class")
+    if runtime.dp_state()[0]:
+        raise RuntimeError("LovaszLoss does not run under data parallelism: its value on the global batch needs one "
+                           "sort over every rank's voxels")
+
+
+def lovasz_scale_size(n: int, c: int, per_image: bool) -> int:
+    return n * c if per_image else c
+
+
+class _LovaszLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, labels, per_image, ignore, owner):
+        c = logits.shape[1]
+        lovasz_check(c)
+        be = runtime.get_backend(logits)
+        z, perm = prepare_logits(logits)
+        t = prepare_labels(labels, c)
+        if t.numel() * c != z.numel():
+            raise RuntimeError(f"label shape {tuple(labels.shape)} does not match logits {tuple(logits.shape)}")
+        dev, n = z.device, z.shape[0]
+        # the per-step accuracy sums come from the fused partial-sum pass of the other losses (its loss sums unused)
+        buf = torch.zeros(be.part_size(c) + n * c * 3, dtype=torch.float64, device=dev)
+        metric = buf[be.part_size(c):].view(n, c, 3)
+        be.loss_partials(z, t, 2.0, 0.25, buf[:be.part_size(c)], metric)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        coef = torch.empty_like(z)
+        scale = torch.empty(lovasz_scale_size(n, c, per_image), dtype=torch.float32, device=dev)
+        be.lovasz_fwd(z, t, per_image, ignore_label(ignore), loss, coef, scale)
+        if owner is not None:
+            owner._metric_sums = metric
+        ctx.save_for_backward(z, t, coef, scale)
+        ctx.per_image = per_image
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        z, t, coef, scale = ctx.saved_tensors
+        be = runtime.get_backend(z)
+        dz = torch.empty_like(z)
+        g = gout.detach().to(torch.float32).reshape(1).contiguous()
+        be.lovasz_bwd(z, t, ctx.per_image, coef, scale, g, dz)
+        inv = (0, 4, 1, 2, 3) if z.dim() == 5 else (0, 3, 1, 2)
+        return dz.permute(*inv), None, None, None, None
 
 
 class _LossBase(nn.Module):
@@ -122,12 +189,18 @@ def loss_spec(lossfn):
     table = {"BinaryDiceLoss": DICE, "BinaryCrossEntropyLoss": CE, "BinaryFocalLoss": FOCAL,
              "BinaryCrossEntropyDiceLoss": DICE | CE, "BinaryDiceFocalLoss": DICE | FOCAL,
              "MutilCrossEntropyLoss": CE, "MutilFocalLoss": FOCAL, "MutilDiceLoss": DICE,
-             "MutilCrossEntropyDiceLoss": DICE | CE}
+             "MutilCrossEntropyDiceLoss": DICE | CE,
+             "BinaryJaccardLoss": JACCARD, "BinaryELDiceLoss": ELDICE, "BinaryTverskyLoss": TVERSKY,
+             "BinarySSLoss": SS, "MutilELDiceLoss": ELDICE, "LovaszLoss": LOVASZ}
     if name not in table:
         raise TypeError(f"{name} is not a pytorchdeeplearing_b200 loss")
-    alpha = getattr(lossfn, "alpha", None) if name.startswith("Mutil") and (table[name] & DICE) else None
+    alpha = getattr(lossfn, "alpha", None) if name.startswith("Mutil") and (table[name] & (DICE | ELDICE)) else None
     gamma = float(getattr(lossfn, "gamma", 2.0))
     alpha_f = float(getattr(lossfn, "alpha", 0.25)) if name in ("BinaryFocalLoss", "BinaryDiceFocalLoss") else 0.25
+    if name == "BinaryTverskyLoss":
+        alpha_f, gamma = float(lossfn.alpha), float(lossfn.beta)
+    elif name == "BinarySSLoss":
+        alpha_f = float(lossfn.r)
     return table[name], alpha, gamma, alpha_f
 
 
@@ -234,6 +307,83 @@ class MutilCrossEntropyDiceLoss(_LossBase):
         return _call(y_pred_logits, y_true, DICE | CE, alpha=self.alpha, owner=self)
 
 
+# ------------------------------------------------------------------------------ further reference losses
+class BinaryJaccardLoss(_LossBase):
+    """reference model/losses.py:9-30"""
+
+    def __init__(self):
+        super().__init__()
+        self.smooth = 1e-5
+        self.eps = 1e-7
+
+    def forward(self, y_pred_logits, y_true):
+        return _call(y_pred_logits, y_true, JACCARD, owner=self)
+
+
+class BinaryELDiceLoss(_LossBase):
+    """reference model/losses.py:56-74: clamp((-log(dsc + smooth))^0.3, 0, 2)"""
+
+    def __init__(self):
+        super().__init__()
+        self.smooth = 1e-5
+        self.eps = 1e-7
+
+    def forward(self, y_pred_logits, y_true):
+        return _call(y_pred_logits, y_true, ELDICE, owner=self)
+
+
+class BinarySSLoss(_LossBase):
+    """reference model/losses.py:77-99 (sensitivity-specificity, weight r)"""
+
+    def __init__(self):
+        super().__init__()
+        self.smooth = 1e-5
+        self.r = 0.1
+
+    def forward(self, y_pred_logits, y_true):
+        return _call(y_pred_logits, y_true, SS, alpha_f=self.r, owner=self)
+
+
+class BinaryTverskyLoss(_LossBase):
+    """reference model/losses.py:102-126: clamp(1 - tversky, 0, 2)"""
+
+    def __init__(self):
+        super().__init__()
+        self.smooth = 1e-5
+        self.alpha = 0.3
+        self.beta = 0.7
+
+    def forward(self, y_pred_logits, y_true):
+        return _call(y_pred_logits, y_true, TVERSKY, gamma=self.beta, alpha_f=self.alpha, owner=self)
+
+
+class MutilELDiceLoss(_LossBase):
+    """reference model/losses.py:345-382: the sum over ALL classes of (-log(d_c present_c alpha_c + smooth))^0.3,
+    divided by the number of present classes, clamped to [0, 2]"""
+
+    def __init__(self, alpha):
+        super().__init__()
+        self.alpha = alpha
+
+    def forward(self, y_pred_logits, y_true):
+        return _call(y_pred_logits, y_true, ELDICE, alpha=self.alpha, owner=self)
+
+
+class LovaszLoss(_LossBase):
+    """reference model/losses.py:462-473 -> model/lovasz.py:90-138 (Lovasz-Softmax over the classes present in the
+    labels).  As in the reference the logits themselves are taken as the probabilities.  Labels outside [0, C) are
+    background for every class; C == 1 raises.  Not available under data parallelism (it needs a global sort)."""
+
+    def __init__(self, per_image=False, ignore=None):
+        super().__init__()
+        self.ignore = ignore
+        self.per_image = per_image
+
+    def forward(self, logits, target):
+        return _LovaszLoss.apply(logits, target, bool(self.per_image), self.ignore, self)
+
+
 __all__ = ["BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
-           "MutilCrossEntropyDiceLoss"]
+           "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
+           "MutilELDiceLoss", "LovaszLoss"]
