@@ -94,6 +94,10 @@ __device__ __forceinline__ void wgmma_fence() {
 }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed groups of this warpgroup are still in flight (N = 1: the previous chain is complete
+// while the one just committed keeps the tensor core busy)
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accesses of the accumulator registers across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
