@@ -48,6 +48,24 @@ extern "C" {
 #define B200SEG_DOWN 2  /* k=2, s=2 convolution (space-to-depth GEMM) */
 #define B200SEG_UP 3    /* k=2, s=2 transposed convolution (GEMM + depth-to-space) */
 
+/* kernel families b200seg_conv chooses from (b200seg_conv_path) */
+#define B200SEG_CONV_PW_MMA 0    /* pw_mma.cu: register-level mma.sync 1x1x1 / transposed conv, >= 65536 voxels */
+#define B200SEG_CONV_TC 1        /* conv_tc.cu: wgmma + TMA implicit GEMM */
+#define B200SEG_CONV_HALO2D 2    /* conv_halo.cu: halo-staged 3x3, 16/32 channels */
+#define B200SEG_CONV_HALO3 3     /* conv_halo.cu: halo-staged 3x3x3, 16/32 channels */
+#define B200SEG_CONV_HALO_WS 4   /* conv_halo_ws.cu: weight-streaming halo-staged 3x3x3, 64/128 input channels */
+#define B200SEG_CONV_STEM_MMA 5  /* stem_mma.cu: one input channel on mma.sync */
+#define B200SEG_CONV_STEM 6      /* stem.cu: one input channel on CUDA cores */
+#define B200SEG_CONV_SMALLCIN 7  /* small_channels.cu: <= 4 input channels */
+#define B200SEG_CONV_GENERIC 8   /* conv_generic.cu: any shape */
+/* kernel families b200seg_wgrad chooses from (b200seg_wgrad_path) */
+#define B200SEG_WGRAD_HALO_MMA 0 /* wgrad_halo_mma.cu: 3x3x3, 16/32 channels, >= 32768 voxels */
+#define B200SEG_WGRAD_TC 1       /* wgrad_tc.cu: wgmma + TMA */
+#define B200SEG_WGRAD_STEM_MMA 2 /* stem_mma.cu */
+#define B200SEG_WGRAD_STEM 3     /* stem.cu */
+#define B200SEG_WGRAD_SMALLCIN 4 /* small_channels.cu */
+#define B200SEG_WGRAD_GENERIC 5  /* wgrad_generic.cu */
+
 /* loss terms (bitmask) */
 #define B200SEG_LOSS_DICE 1
 #define B200SEG_LOSS_CE 2
@@ -115,6 +133,10 @@ int b200seg_unpack_wgrads_multi(const b200seg_pack_desc* table, int count, int t
 int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, int w_dtype, const float* bias,
                  const b200seg_tensor* y, double* stats, const b200seg_tensor* addend, int device,
                  b200seg_stream stream);
+/* the B200SEG_CONV_* kernel family b200seg_conv would run for these arguments (host only, launches nothing), or
+ * B200SEG_EINVAL where b200seg_conv would refuse them */
+int b200seg_conv_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
+                      const b200seg_tensor* addend);
 
 /* Data-gradient convolution that ALSO accumulates the GroupNorm-backward sums of the layer behind its output:
  * g = conv_kind(x, wpk) [+ addend] is dL/d(activation) of the layer whose raw conv output is `yfwd` and whose
@@ -146,6 +168,8 @@ int b200seg_conv_halo_ws_ntile(int kind, int cin, int cout);
  * kind in {K3, K1, DOWN}; for the transposed conv call with kind = DOWN, a = dy (fine), b = x. */
 int b200seg_wgrad(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b, float* dwp, int device,
                   b200seg_stream stream);
+/* the B200SEG_WGRAD_* kernel family b200seg_wgrad would run for these arguments (host only), or B200SEG_EINVAL */
+int b200seg_wgrad_path(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b);
 
 /* ---- GroupNorm(8) + Dropout(p) + ReLU tail (nn.GroupNorm / nn.Dropout3d / nn.ReLU, VNet3d.py:9-11,14;
  * Unet3d.py:73-75) split into statistics (conv epilogue) -> finalize -> apply (SURVEY.md App. G) */

@@ -16,6 +16,9 @@ import torch
 K3, K1, DOWN, UP = 0, 1, 2, 3
 F32, BF16, BF16_TC, BF16_HALO, BF16_HALO_WS = 0, 1, 2, 3, 4
 I64 = 16
+# kernel families of b200seg_conv / b200seg_wgrad (include/b200seg.h: B200SEG_CONV_*, B200SEG_WGRAD_*)
+CONV_PATHS = ("PW_MMA", "TC", "HALO2D", "HALO3", "HALO_WS", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
+WGRAD_PATHS = ("HALO_MMA", "TC", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
 # voxels per sample a 3x3x3 layer needs before its weights are packed for the halo-staged kernels (16/32 channels)
 # and the weight-streaming halo kernel (64/128 channels); smaller layers take the TMA implicit-GEMM kernel
 HALO_MIN_VOX = 128 * 128
@@ -55,12 +58,14 @@ _SIGNATURES = {
     "b200seg_unpack_wgrads_multi": ([_vp, _i, _i, _i, _vp], C.c_int),
     "b200seg_upload_table": ([_vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_conv": ([_i, _i, _PT, _vp, _i, _vp, _PT, _vp, _PT, _i, _vp], C.c_int),
+    "b200seg_conv_path": ([_i, _i, _PT, _i, _PT, _PT], C.c_int),
     "b200seg_conv_bwdstats_supported": ([_i, _i, _PT, _i, _PT, _PT, _PT], C.c_int),
     "b200seg_conv_bwdstats": ([_i, _i, _PT, _vp, _i, _PT, _PT, _PT, _PG, _vp, _i, _vp], C.c_int),
     "b200seg_conv_tc_eligible": ([_i, _i, _i], C.c_int),
     "b200seg_conv_halo_eligible": ([_i, _i, _i], C.c_int),
     "b200seg_conv_halo_ws_ntile": ([_i, _i, _i], C.c_int),
     "b200seg_wgrad": ([_i, _i, _PT, _PT, _vp, _i, _vp], C.c_int),
+    "b200seg_wgrad_path": ([_i, _i, _PT, _PT], C.c_int),
     "b200seg_gn_finalize": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i64, _f, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_apply": ([_PT, _vp, _PT, _vp, _PT, _PT, _i, _vp], C.c_int),
     "b200seg_apply_gn": ([_PT, _PG, _PT, _PG, _PT, _PT, _i, _vp], C.c_int),
@@ -357,14 +362,36 @@ class CudaBackend:
         self._check(self.lib.b200seg_unpack_wgrad(dwp.data_ptr(), grad.data_ptr(), t, k, n, 1, t, k * t, dev, st))
 
     # ------------------------------------------------------------------ conv family
+    @staticmethod
+    def _needs_repack(wpk, x, y):
+        # the wgmma paths need bf16 activations on both sides (e.g. a 16-channel fp32 network input)
+        return wpk.code in (BF16_TC, BF16_HALO, BF16_HALO_WS) and not (x.dtype == torch.bfloat16 and
+                                                                      y.dtype == torch.bfloat16)
+
     def conv(self, kind, dims, x, wpk, bias, y, stats, addend):
         dev, st = self._ds(x)
-        if wpk.code in (BF16_TC, BF16_HALO, BF16_HALO_WS) and not (x.dtype == torch.bfloat16 and y.dtype == torch.bfloat16):
-            # wgmma path needs bf16 activations on both sides (e.g. a 16-channel fp32 network input)
+        if self._needs_repack(wpk, x, y):
             wpk = self.pack_weight(wpk.src, wpk.kind, wpk.which, torch.bfloat16, wpk.dims, allow_tc=False)
         dx, dy, da = _desc(x), _desc(y), _desc(addend)
         self._check(self.lib.b200seg_conv(kind, dims, C.byref(dx), wpk.t.data_ptr(), wpk.code, _p(bias), C.byref(dy),
                                           _p(stats), _ref(da), dev, st))
+
+    def conv_path(self, kind, dims, x, wpk, y, addend=None):
+        """name (CONV_PATHS) of the kernel family ``conv`` would launch for these arguments; launches nothing"""
+        code = BF16 if self._needs_repack(wpk, x, y) else wpk.code
+        dx, dy, da = _desc(x), _desc(y), _desc(addend)
+        rc = self.lib.b200seg_conv_path(kind, dims, C.byref(dx), code, C.byref(dy), _ref(da))
+        if rc < 0:
+            raise RuntimeError(f"libb200seg error {rc}: {self.lib.b200seg_last_error().decode()}")
+        return CONV_PATHS[rc]
+
+    def wgrad_path(self, kind, dims, a, b):
+        """name (WGRAD_PATHS) of the kernel family ``wgrad`` would launch for these arguments; launches nothing"""
+        da, db = _desc(a), _desc(b)
+        rc = self.lib.b200seg_wgrad_path(kind, dims, C.byref(da), C.byref(db))
+        if rc < 0:
+            raise RuntimeError(f"libb200seg error {rc}: {self.lib.b200seg_last_error().decode()}")
+        return WGRAD_PATHS[rc]
 
     def conv_bwdstats_ok(self, kind, dims, x, wpk, y, addend, yfwd):
         """can ``conv_bwdstats`` take this data-gradient convolution (3-D halo-staged 16/32-channel 3x3x3 layers)?"""

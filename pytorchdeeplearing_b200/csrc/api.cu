@@ -194,6 +194,38 @@ int b200seg_unpack_wgrads_multi(const b200seg_pack_desc* table, int count, int t
   return ew_pack_multi(table, count, total_blocks, 1, ST(stream));
 }
 
+// The kernel family b200seg_conv runs, from the arguments alone (x, y, addend already validated).  b200seg_conv
+// switches on this value, so the query and the launch cannot disagree.
+static int conv_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
+                     const b200seg_tensor* addend) {
+  if (pw_mma_supported(kind, dims, x, w_dtype, y, addend)) return B200SEG_CONV_PW_MMA;
+  if (conv_tc_supported(kind, dims, x, w_dtype, y, addend)) return B200SEG_CONV_TC;
+  if (conv_halo_supported(kind, dims, x, w_dtype, y, addend))
+    return dims == 3 ? B200SEG_CONV_HALO3 : B200SEG_CONV_HALO2D;
+  if (conv_halows_supported(kind, dims, x, w_dtype, y, addend)) return B200SEG_CONV_HALO_WS;
+  if (w_dtype == B200SEG_BF16_TC || w_dtype == B200SEG_BF16_HALO || w_dtype == B200SEG_BF16_HALO_WS)
+    return B200SEG_EINVAL;
+  const bool small_types =
+      w_dtype == B200SEG_F32 ? (x->dtype == B200SEG_F32 && y->dtype == B200SEG_F32) : y->dtype == B200SEG_BF16;
+  if (stem_mma_conv_supported(kind, x, w_dtype, y, addend)) return B200SEG_CONV_STEM_MMA;
+  if (small_types && stem_conv_supported(kind, x, y, addend)) return B200SEG_CONV_STEM;
+  if (small_types && smallcin_conv_supported(kind, x, y, addend)) return B200SEG_CONV_SMALLCIN;
+  return B200SEG_CONV_GENERIC;
+}
+
+int b200seg_conv_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
+                      const b200seg_tensor* addend) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(y, "y");
+  OPT_TENSOR(addend, "addend");
+  B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_conv_path: dims must be 2 or 3");
+  B200_CHECK_ARG(dims == 3 || (x->d == 1 && y->d == 1), "b200seg_conv_path: 2-D tensors must have d == 1");
+  const int path = conv_path(kind, dims, x, w_dtype, y, addend);
+  B200_CHECK_ARG(path >= 0, "b200seg_conv_path: packed tensor-core weights need bf16, 16-byte aligned activations of "
+                 "a supported shape");
+  return path;
+}
+
 int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, int w_dtype, const float* bias,
                  const b200seg_tensor* y, double* stats, const b200seg_tensor* addend, int device,
                  b200seg_stream stream) {
@@ -204,45 +236,37 @@ int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, i
   B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_conv: dims must be 2 or 3");
   B200_CHECK_ARG(dims == 3 || (x->d == 1 && y->d == 1), "b200seg_conv: 2-D tensors must have d == 1");
   B200_DEVICE(device);
-  if (pw_mma_supported(kind, dims, x, w_dtype, y, addend))
-    return pw_mma_conv(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
-  if (conv_tc_supported(kind, dims, x, w_dtype, y, addend))
-    return conv_tc(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
-  if (conv_halo_supported(kind, dims, x, w_dtype, y, addend)) {
-    if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
-    return conv_halo(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
+  switch (conv_path(kind, dims, x, w_dtype, y, addend)) {
+    case B200SEG_CONV_PW_MMA:
+      return pw_mma_conv(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
+    case B200SEG_CONV_TC:
+      return conv_tc(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
+    case B200SEG_CONV_HALO2D:
+    case B200SEG_CONV_HALO3:
+      if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
+      return conv_halo(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
+    case B200SEG_CONV_HALO_WS:
+      if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
+      return conv_halows(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
+    case B200SEG_CONV_STEM_MMA:
+      return stem_mma_conv(kind, dims, x, wpk, bias, y, stats, device, ST(stream));
+    case B200SEG_CONV_STEM:
+      return stem_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
+    case B200SEG_CONV_SMALLCIN:
+      return smallcin_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
+    case B200SEG_CONV_GENERIC:
+      return conv_generic(kind, dims, x, wpk, w_dtype, bias, y, stats, addend, ST(stream));
   }
-  if (conv_halows_supported(kind, dims, x, w_dtype, y, addend)) {
-    if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
-    return conv_halows(kind, dims, x, wpk, bias, y, stats, addend, device, ST(stream));
-  }
-  B200_CHECK_ARG(w_dtype != B200SEG_BF16_TC && w_dtype != B200SEG_BF16_HALO && w_dtype != B200SEG_BF16_HALO_WS,
-                 "b200seg_conv: B200SEG_BF16_TC weights need bf16, 16-byte aligned activations of a supported shape");
-  const bool small_types =
-      w_dtype == B200SEG_F32 ? (x->dtype == B200SEG_F32 && y->dtype == B200SEG_F32) : y->dtype == B200SEG_BF16;
-  if (stem_mma_conv_supported(kind, x, w_dtype, y, addend))
-    return stem_mma_conv(kind, dims, x, wpk, bias, y, stats, device, ST(stream));
-  if (small_types && stem_conv_supported(kind, x, y, addend))
-    return stem_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
-  if (small_types && smallcin_conv_supported(kind, x, y, addend))
-    return smallcin_conv(kind, dims, x, wpk, w_dtype, bias, y, stats, device, ST(stream));
-  return conv_generic(kind, dims, x, wpk, w_dtype, bias, y, stats, addend, ST(stream));
-}
-
-static int bwdstats_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
-                         const b200seg_tensor* addend) {
-  // 1: halo3 (16/32 channels, 3-D), 2: halo-ws (64/128 channels), 0: none -- and only where b200seg_conv itself would
-  // take that kernel
-  if (pw_mma_supported(kind, dims, x, w_dtype, y, addend) || conv_tc_supported(kind, dims, x, w_dtype, y, addend)) return 0;
-  if (conv_halo_supported(kind, dims, x, w_dtype, y, addend)) return dims == 3 ? 1 : 0;
-  if (conv_halows_supported(kind, dims, x, w_dtype, y, addend)) return 2;
-  return 0;
+  set_error("b200seg_conv: B200SEG_BF16_TC weights need bf16, 16-byte aligned activations of a supported shape");
+  return B200SEG_EINVAL;
 }
 
 int b200seg_conv_bwdstats_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                                     const b200seg_tensor* addend, const b200seg_tensor* yfwd) {
   if (x == nullptr || y == nullptr || yfwd == nullptr) return 0;
-  if (bwdstats_path(kind, dims, x, w_dtype, y, addend) == 0) return 0;
+  // only where b200seg_conv itself takes a kernel with the backward-sums epilogue
+  const int path = conv_path(kind, dims, x, w_dtype, y, addend);
+  if (path != B200SEG_CONV_HALO3 && path != B200SEG_CONV_HALO_WS) return 0;
   return (yfwd->n == y->n && yfwd->d == y->d && yfwd->h == y->h && yfwd->w == y->w && yfwd->c == y->c &&
           yfwd->dtype == B200SEG_BF16 && (yfwd->ld % 8) == 0 && (reinterpret_cast<uintptr_t>(yfwd->ptr) % 16) == 0)
              ? 1 : 0;
@@ -261,7 +285,7 @@ int b200seg_conv_bwdstats(int kind, int dims, const b200seg_tensor* x, const voi
                  "b200seg_conv_bwdstats: unsupported shape (query b200seg_conv_bwdstats_supported first)");
   B200_DEVICE(device);
   if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
-  if (bwdstats_path(kind, dims, x, w_dtype, y, addend) == 2)
+  if (conv_path(kind, dims, x, w_dtype, y, addend) == B200SEG_CONV_HALO_WS)
     return conv_halows(kind, dims, x, wpk, nullptr, y, nullptr, addend, device, ST(stream), yfwd, gn, sums);
   return conv_halo(kind, dims, x, wpk, nullptr, y, nullptr, addend, device, ST(stream), yfwd, gn, sums);
 }
@@ -272,6 +296,16 @@ int b200seg_conv_halo_eligible(int kind, int cin, int cout) { return conv_halo_c
 
 int b200seg_conv_halo_ws_ntile(int kind, int cin, int cout) { return conv_halows_ntile(kind, cin, cout); }
 
+// the kernel family b200seg_wgrad runs (a, b already validated); b200seg_wgrad switches on it
+static int wgrad_path(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b) {
+  if (wgrad_halo_mma_supported(kind, dims, a, b)) return B200SEG_WGRAD_HALO_MMA;
+  if (wgrad_tc_supported(kind, dims, a, b)) return B200SEG_WGRAD_TC;
+  if (stem_mma_wgrad_supported(kind, a, b)) return B200SEG_WGRAD_STEM_MMA;
+  if (stem_wgrad_supported(kind, a, b)) return B200SEG_WGRAD_STEM;
+  if (smallcin_wgrad_supported(kind, a, b)) return B200SEG_WGRAD_SMALLCIN;
+  return B200SEG_WGRAD_GENERIC;
+}
+
 int b200seg_wgrad(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b, float* dwp, int device,
                   b200seg_stream stream) {
   REQ_TENSOR(a, "a");
@@ -279,17 +313,28 @@ int b200seg_wgrad(int kind, int dims, const b200seg_tensor* a, const b200seg_ten
   B200_CHECK_ARG(dwp != nullptr, "b200seg_wgrad: null output");
   B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_wgrad: dims must be 2 or 3");
   B200_DEVICE(device);
-  if (wgrad_halo_mma_supported(kind, dims, a, b))
-    return wgrad_halo_mma(kind, dims, a, b, dwp, device, ST(stream));
-  if (wgrad_tc_supported(kind, dims, a, b)) {
-    if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
-    return wgrad_tc(kind, dims, a, b, dwp, device, ST(stream));
+  switch (wgrad_path(kind, dims, a, b)) {
+    case B200SEG_WGRAD_HALO_MMA:
+      return wgrad_halo_mma(kind, dims, a, b, dwp, device, ST(stream));
+    case B200SEG_WGRAD_TC:
+      if (conv_tc_init(device) != B200SEG_OK) return B200SEG_ECUDA;
+      return wgrad_tc(kind, dims, a, b, dwp, device, ST(stream));
+    case B200SEG_WGRAD_STEM_MMA:
+      return stem_mma_wgrad(kind, dims, a, b, dwp, device, ST(stream));
+    case B200SEG_WGRAD_STEM:
+      return stem_wgrad(kind, dims, a, b, dwp, device, ST(stream));
+    case B200SEG_WGRAD_SMALLCIN:
+      return smallcin_wgrad(kind, dims, a, b, dwp, device, ST(stream));
+    default:
+      return wgrad_generic(kind, dims, a, b, dwp, device, ST(stream));
   }
-  if (stem_mma_wgrad_supported(kind, a, b))
-    return stem_mma_wgrad(kind, dims, a, b, dwp, device, ST(stream));
-  if (stem_wgrad_supported(kind, a, b)) return stem_wgrad(kind, dims, a, b, dwp, device, ST(stream));
-  if (smallcin_wgrad_supported(kind, a, b)) return smallcin_wgrad(kind, dims, a, b, dwp, device, ST(stream));
-  return wgrad_generic(kind, dims, a, b, dwp, device, ST(stream));
+}
+
+int b200seg_wgrad_path(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b) {
+  REQ_TENSOR(a, "a");
+  REQ_TENSOR(b, "b");
+  B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_wgrad_path: dims must be 2 or 3");
+  return wgrad_path(kind, dims, a, b);
 }
 
 int b200seg_gn_finalize(const double* stats, const float* gamma, const float* beta, const float* scale, int N, int C,
