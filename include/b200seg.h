@@ -41,6 +41,8 @@ extern "C" {
                                   per-group tap blocks streamed by the 64/128-channel halo-staged 3x3x3 path */
 
 #define B200SEG_I64 16 /* labels only: int64 class indices (model/dataset.py:114); B200SEG_F32 = soft binary targets */
+#define B200SEG_U8 17  /* masks only: one byte per voxel (bool or uint8) */
+#define B200SEG_I32 18 /* masks only: int32 */
 
 /* conv kinds */
 #define B200SEG_K3 0    /* 3x3x3 (dims==3) or 1x3x3 (dims==2), stride 1, zero pad 1 */
@@ -303,6 +305,30 @@ int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_
 int b200seg_metric_partials(const float* probs, const void* labels, int label_dtype, int N, int64_t vox_per_sample,
                             int C, float threshold, double* metric, int device, b200seg_stream stream);
 int b200seg_metric_finalize(const double* metric, int N, int C, float* out /*[2]*/, int device, b200seg_stream stream);
+
+/* ---- 3-D segmentation metrics of Seg_Metirc3d (model/metric.py:11-142; scipy binary_erosion + cKDTree there) for N
+ * volumes of (D, H, W) voxels.  real / pred: dense [N][D][H][W] masks of dtype B200SEG_U8 (bool, uint8), B200SEG_I32
+ * or B200SEG_I64; nonzero is foreground.  spacing_zyx: DEVICE fp64 [N][3] (z, y, x) in mm, the reversed SimpleITK
+ * spacing (metric.py:47).  A surface voxel is a foreground voxel with background in its 18-neighbourhood (faces and
+ * edges; outside the volume is background: metric.py:41-42).  Distances are exact Euclidean distances in mm from each
+ * surface voxel to the nearest surface voxel of the other mask (metric.py:49-65), from a separable exact distance
+ * transform in fp64.
+ * b200seg_segmetric3d writes counts int64 [N][6] = {R, P, I, U, S_r, S_p} (foreground, intersection, union and surface
+ * voxel counts), metrics fp64 [N][9] = {dice 2I/(R+P), jaccard I/U, VOE 1 - I/U, RVD (P-R)/R, FNR (R-I)/U,
+ * FPR (P-I)/U, ASSD, RMSD, MSD} (metric.py:68-142; distance metrics NaN where a mask is empty) and flags int32 [N]
+ * (1 where a mask holds a value outside {0, 1}).  Every reduction has a fixed order: reruns are bit-identical.
+ * b200seg_segmetric3d_points writes, for each surface in C order over all volumes (volume n's points follow those of
+ * volumes < n, counts from b200seg_segmetric3d), the linear voxel index within the volume (metric.py:43-44) and the
+ * distance to the other surface (real2pred_nn / pred2real_nn, metric.py:58-65); at most cap_r / cap_p points are
+ * written.  Both take a workspace of b200seg_segmetric3d_workspace(N, D, H, W) bytes (about 65 bytes per voxel). */
+int64_t b200seg_segmetric3d_workspace(int N, int D, int H, int W);
+int b200seg_segmetric3d(const void* real, int real_dtype, const void* pred, int pred_dtype, int N, int D, int H, int W,
+                        const double* spacing_zyx, void* workspace, int64_t workspace_bytes, int64_t* counts,
+                        double* metrics, int32_t* flags, int device, b200seg_stream stream);
+int b200seg_segmetric3d_points(const void* real, int real_dtype, const void* pred, int pred_dtype, int N, int D, int H,
+                               int W, const double* spacing_zyx, void* workspace, int64_t workspace_bytes,
+                               int64_t cap_r, int64_t cap_p, int64_t* real_idx, int64_t* pred_idx, double* real2pred,
+                               double* pred2real, int device, b200seg_stream stream);
 
 /* ---- fused optimizer step over FLAT fp32 buffers (torch.optim.AdamW(lr) model/modelVNet.py:548, weight_decay 0.01,
  * decoupled = 1; torch.optim.Adam model/modelUnet.py:849, decoupled = 0): ONE launch for all parameters instead of

@@ -1,7 +1,8 @@
 """pytorchdeeplearing_b200 -- H100-native (sm_90a) drop-in for the segmentation hot path of
 junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
 ``networks/Unet2d.py`` forward/backward and the losses of ``model/losses.py`` (Dice / BCE / focal / CE,
-Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8).
+Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8), and the
+3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -18,12 +19,13 @@ from .losses import (BinaryDiceLoss, BinaryCrossEntropyLoss, BinaryFocalLoss, Bi
 from .install import install, uninstall
 from .graphed import GraphedStep
 from .optim import FusedAdamW, FusedAdam
-from .metric import dice_coeff, iou_coeff, multiclass_dice_coeff, multiclass_iou_coeff
+from .metric import dice_coeff, iou_coeff, multiclass_dice_coeff, multiclass_iou_coeff, seg_metrics3d, Seg_Metirc3d
 from .inference import predict, predict_mask, sliding_window_mask
 from .staging import InputStager, stage_batch
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
-           "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "predict", "predict_mask",
+           "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
+           "predict_mask",
            "sliding_window_mask", "InputStager", "stage_batch", "set_precision", "get_precision",
            "enable_data_parallel", "disable_data_parallel", "install", "uninstall", "GraphedStep",
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",

@@ -16,6 +16,7 @@ import torch
 K3, K1, DOWN, UP = 0, 1, 2, 3
 F32, BF16, BF16_TC, BF16_HALO, BF16_HALO_WS = 0, 1, 2, 3, 4
 I64 = 16
+U8, I32 = 17, 18          # mask dtypes of the segmentation metrics
 # kernel families of b200seg_conv / b200seg_wgrad (include/b200seg.h: B200SEG_CONV_*, B200SEG_WGRAD_*)
 CONV_PATHS = ("PW_MMA", "TC", "HALO2D", "HALO3", "HALO_WS", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
 WGRAD_PATHS = ("HALO_MMA", "TC", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
@@ -93,6 +94,10 @@ _SIGNATURES = {
     "b200seg_lovasz_workspace": ([_i, _i64, _i, _i], C.c_int64),
     "b200seg_lovasz_fwd": ([_vp, _vp, _i, _i64, _i, _i, _i, _i64, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_lovasz_bwd": ([_vp, _vp, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_segmetric3d_workspace": ([_i, _i, _i, _i], C.c_int64),
+    "b200seg_segmetric3d": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_segmetric3d_points": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp,
+                                    _i, _vp], C.c_int),
     "b200seg_metric_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _vp, _i, _vp], C.c_int),
     "b200seg_metric_finalize": ([_vp, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _i, _i, _vp], C.c_int),
@@ -610,6 +615,36 @@ class CudaBackend:
         self._check(self.lib.b200seg_lovasz_bwd(logits.data_ptr(), labels.data_ptr(), n, logits.numel() // (n * c), c,
                                                 1 if per_image else 0, coef.data_ptr(), seg_scale.data_ptr(),
                                                 gscale.data_ptr(), dlogits.data_ptr(), dev, st))
+
+    # ------------------------------------------------------------------ 3-D segmentation metrics (model/metric.py:11-142)
+    _MASK_DTYPES = {torch.bool: U8, torch.uint8: U8, torch.int32: I32, torch.int64: I64}
+
+    def _segmetric_args(self, real, pred, spacing_zyx):
+        """real, pred (N, D, H, W) contiguous masks of one shape; spacing_zyx fp64 (N, 3) on the same device"""
+        assert real.shape == pred.shape and real.dim() == 4 and real.is_contiguous() and pred.is_contiguous()
+        assert spacing_zyx.dtype == torch.float64 and spacing_zyx.is_contiguous() and spacing_zyx.numel() >= 3 * real.shape[0]
+        rdt, pdt = self._MASK_DTYPES.get(real.dtype), self._MASK_DTYPES.get(pred.dtype)
+        if rdt is None or pdt is None:
+            raise TypeError(f"masks must be bool, uint8, int32 or int64, got {real.dtype} / {pred.dtype}")
+        n, d, h, w = real.shape
+        nb = int(self.lib.b200seg_segmetric3d_workspace(n, d, h, w))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=real.device)
+        return (real.data_ptr(), rdt, pred.data_ptr(), pdt, n, d, h, w, spacing_zyx.data_ptr(), ws.data_ptr(), nb), ws
+
+    def segmetric3d(self, real, pred, spacing_zyx, counts, metrics, flags):
+        """counts int64 [N][6] = {R, P, I, U, S_r, S_p}, metrics fp64 [N][9] (Seg_Metirc3d's order), flags int32 [N]"""
+        dev, st = self._ds(real)
+        args, ws = self._segmetric_args(real, pred, spacing_zyx)
+        self._check(self.lib.b200seg_segmetric3d(*args, counts.data_ptr(), metrics.data_ptr(), flags.data_ptr(), dev, st))
+
+    def segmetric3d_points(self, real, pred, spacing_zyx, real_idx, pred_idx, real2pred, pred2real):
+        """C-order linear voxel indices of both surfaces (int64) and each point's distance to the other surface (fp64);
+        the four outputs are sized from the surface counts of ``segmetric3d``"""
+        dev, st = self._ds(real)
+        args, ws = self._segmetric_args(real, pred, spacing_zyx)
+        self._check(self.lib.b200seg_segmetric3d_points(*args, real_idx.numel(), pred_idx.numel(), real_idx.data_ptr(),
+                                                        pred_idx.data_ptr(), real2pred.data_ptr(), pred2real.data_ptr(),
+                                                        dev, st))
 
     # ------------------------------------------------------------------ per-step accuracy (model/metric.py)
     def metric_partials(self, probs, labels, threshold, metric):

@@ -134,6 +134,14 @@ int lovasz_fwd(const float* z, const long long* t, int N, long long vox, int C, 
                cudaStream_t s);
 int lovasz_bwd(const float* z, const long long* t, int N, long long vox, int C, int per_image, const float* coef,
                const float* seg_scale, const float* gscale, float* dz, int device, cudaStream_t s);
+int64_t segmetric3d_workspace(int N, int D, int H, int W);
+int segmetric3d(const void* real, int rdt, const void* pred, int pdt, int N, int D, int H, int W,
+                const double* spacing, void* ws, long long ws_bytes, long long* counts, double* metrics, int* flags,
+                int device, cudaStream_t s);
+int segmetric3d_points(const void* real, int rdt, const void* pred, int pdt, int N, int D, int H, int W,
+                       const double* spacing, void* ws, long long ws_bytes, long long cap_r, long long cap_p,
+                       long long* real_idx, long long* pred_idx, double* real_nn, double* pred_nn, int device,
+                       cudaStream_t s);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -641,6 +649,33 @@ int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_
   B200_DEVICE(device);
   return lovasz_bwd(logits, reinterpret_cast<const long long*>(labels), N, vox, C, per_image, coef, seg_scale, gscale,
                     dlogits, device, ST(stream));
+}
+
+int64_t b200seg_segmetric3d_workspace(int N, int D, int H, int W) {
+  if (N < 1 || D < 1 || H < 1 || W < 1) return 0;
+  return segmetric3d_workspace(N, D, H, W);
+}
+
+int b200seg_segmetric3d(const void* real, int real_dtype, const void* pred, int pred_dtype, int N, int D, int H, int W,
+                        const double* spacing_zyx, void* workspace, int64_t workspace_bytes, int64_t* counts,
+                        double* metrics, int32_t* flags, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(real && pred && spacing_zyx && counts && metrics && flags, "b200seg_segmetric3d: null argument");
+  B200_DEVICE(device);
+  return segmetric3d(real, real_dtype, pred, pred_dtype, N, D, H, W, spacing_zyx, workspace, workspace_bytes,
+                     reinterpret_cast<long long*>(counts), metrics, flags, device, ST(stream));
+}
+
+int b200seg_segmetric3d_points(const void* real, int real_dtype, const void* pred, int pred_dtype, int N, int D, int H,
+                               int W, const double* spacing_zyx, void* workspace, int64_t workspace_bytes,
+                               int64_t cap_r, int64_t cap_p, int64_t* real_idx, int64_t* pred_idx, double* real2pred,
+                               double* pred2real, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(real && pred && spacing_zyx, "b200seg_segmetric3d_points: null argument");
+  B200_CHECK_ARG((cap_r == 0 || (real_idx && real2pred)) && (cap_p == 0 || (pred_idx && pred2real)),
+                 "b200seg_segmetric3d_points: null output");
+  B200_DEVICE(device);
+  return segmetric3d_points(real, real_dtype, pred, pred_dtype, N, D, H, W, spacing_zyx, workspace, workspace_bytes,
+                            cap_r, cap_p, reinterpret_cast<long long*>(real_idx),
+                            reinterpret_cast<long long*>(pred_idx), real2pred, pred2real, device, ST(stream));
 }
 
 }  // extern "C"

@@ -13,7 +13,7 @@ import sys
 _SAVED = []
 
 _NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet2d")
-_METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff")
+_METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "Seg_Metirc3d")
 _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
 # the further model/losses.py classes (bound there, not imported by the wrappers)
