@@ -330,6 +330,32 @@ int b200seg_segmetric3d_points(const void* real, int real_dtype, const void* pre
                                int64_t cap_r, int64_t cap_p, int64_t* real_idx, int64_t* pred_idx, double* real2pred,
                                double* pred2real, int device, b200seg_stream stream);
 
+/* ---- SSIM / SSIM3D (model/lossesSSIM.py:49-93: five depthwise F.conv2d / F.conv3d with a dense Gaussian window
+ * there).  img1, img2: fp32 (N, C, H, W) (dims == 2; pass D = 1) or (N, C, D, H, W) with element strides
+ * {n, c, d, h, w} (host int64 [5], read during the call; NCDHW-contiguous and channels-last views alike).  taps: the
+ * window_size (1..31) 1-D Gaussian taps of lossesSSIM.py:28-30 (host fp32, read during the call), applied separably
+ * along H, W (and D) with zero padding P = window_size / 2, so each map axis has length L + 2P - window_size + 1.
+ * The map S (lossesSSIM.py:52-64, 73-88) is formed per voxel in fp64.
+ * b200seg_ssim_fwd writes fp64 partial sums of S into `workspace` (b200seg_ssim_workspace bytes) and, when coef is
+ * not NULL, the four backward coefficients fp64 [4][N][C][D'][H'][W'] = {dS/dmu1, dS/dmu2, dS/dm11 = dS/dm22, dS/dm12}.
+ * b200seg_ssim_finalize sums the partials in a fixed order (reduce != 0) into acc: size_average: acc[2] = {sum S,
+ * count}, value[1] = S.mean(); otherwise per sample, dims == 2: acc[N], value[N] = S.mean(1).mean(1).mean(1); dims ==
+ * 3: acc[N][W'], value[N][W'] (the reference's three means run over C, D and H only).  With reduce == 0 it only
+ * recomputes value from acc (after a data-parallel all-reduce of acc).
+ * b200seg_ssim_bwd: grad1 / grad2 (fp32 NCDHW-contiguous, either may be NULL) = d loss / d img from gout (fp32, the
+ * shape of value) and the forward's coef and acc (the mean's count is read from acc[1]). */
+int64_t b200seg_ssim_workspace(int dims, int N, int C, int D, int H, int W, int window_size);
+int b200seg_ssim_fwd(int dims, const float* img1, const int64_t* strides1, const float* img2, const int64_t* strides2,
+                     int N, int C, int D, int H, int W, int window_size, const float* taps, double* coef,
+                     void* workspace, int64_t workspace_bytes, int device, b200seg_stream stream);
+int b200seg_ssim_finalize(int dims, int N, int C, int D, int H, int W, int window_size, int size_average, int reduce,
+                          const void* workspace, int64_t workspace_bytes, double* acc, float* value, int device,
+                          b200seg_stream stream);
+int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const float* img2, const int64_t* strides2,
+                     int N, int C, int D, int H, int W, int window_size, const float* taps, const double* coef,
+                     int size_average, const float* gout, const double* acc, float* grad1, float* grad2, int device,
+                     b200seg_stream stream);
+
 /* ---- fused optimizer step over FLAT fp32 buffers (torch.optim.AdamW(lr) model/modelVNet.py:548, weight_decay 0.01,
  * decoupled = 1; torch.optim.Adam model/modelUnet.py:849, decoupled = 0): ONE launch for all parameters instead of
  * ~6 foreach launches over 128 tensors.  state (fp32 [4], device): [0] step count t, [1] lr/(1-b1^t), [2]

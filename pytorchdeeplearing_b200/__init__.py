@@ -2,7 +2,8 @@
 junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
 ``networks/Unet2d.py`` forward/backward and the losses of ``model/losses.py`` (Dice / BCE / focal / CE,
 Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8), and the
-3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``).
+3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``) and the SSIM losses of
+``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -22,6 +23,7 @@ from .optim import FusedAdamW, FusedAdam
 from .metric import dice_coeff, iou_coeff, multiclass_dice_coeff, multiclass_iou_coeff, seg_metrics3d, Seg_Metirc3d
 from .inference import predict, predict_mask, sliding_window_mask
 from .staging import InputStager, stage_batch
+from .ssim import SSIM, SSIM3D, ssim, ssim3D
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
@@ -31,4 +33,4 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "initialize_weights", "FusedA
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
            "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
-           "MutilELDiceLoss", "LovaszLoss"]
+           "MutilELDiceLoss", "LovaszLoss", "SSIM", "SSIM3D", "ssim", "ssim3D"]

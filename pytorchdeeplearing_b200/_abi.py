@@ -98,6 +98,11 @@ _SIGNATURES = {
     "b200seg_segmetric3d": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_segmetric3d_points": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp,
                                     _i, _vp], C.c_int),
+    "b200seg_ssim_workspace": ([_i, _i, _i, _i, _i, _i, _i], C.c_int64),
+    "b200seg_ssim_fwd": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _i, _vp], C.c_int),
+    "b200seg_ssim_finalize": ([_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i64, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_ssim_bwd": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp],
+                         C.c_int),
     "b200seg_metric_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _vp, _i, _vp], C.c_int),
     "b200seg_metric_finalize": ([_vp, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _i, _i, _vp], C.c_int),
@@ -645,6 +650,50 @@ class CudaBackend:
         self._check(self.lib.b200seg_segmetric3d_points(*args, real_idx.numel(), pred_idx.numel(), real_idx.data_ptr(),
                                                         pred_idx.data_ptr(), real2pred.data_ptr(), pred2real.data_ptr(),
                                                         dev, st))
+
+    # ------------------------------------------------------------------ SSIM / SSIM3D (model/lossesSSIM.py:49-93)
+    @staticmethod
+    def _ssim_geom(img):
+        """(dims, N, C, D, H, W) and the host {n, c, d, h, w} element strides of an fp32 (N,C,H,W) / (N,C,D,H,W) image"""
+        if img.dim() == 4:
+            n, c, h, w = img.shape
+            sn, sc, sh, sw = img.stride()
+            return (2, n, c, 1, h, w), (C.c_int64 * 5)(sn, sc, 0, sh, sw)
+        return (3,) + tuple(img.shape), (C.c_int64 * 5)(*img.stride())
+
+    def ssim_fwd(self, img1, img2, window_size, taps, coef):
+        """img1, img2 fp32 of one shape, any strides; taps fp32 host [window_size]; coef fp64 [4][map voxels] or None.
+        -> the workspace holding the partial sums of the map (input of ssim_finalize)"""
+        dev, st = self._ds(img1)
+        geom, s1 = self._ssim_geom(img1)
+        _, s2 = self._ssim_geom(img2)
+        nb = int(self.lib.b200seg_ssim_workspace(*geom, window_size))
+        ws = torch.empty(max(nb, 8) // 8, dtype=torch.float64, device=img1.device)
+        t = (C.c_float * window_size)(*[float(v) for v in taps])
+        self._check(self.lib.b200seg_ssim_fwd(geom[0], img1.data_ptr(), C.cast(s1, _vp), img2.data_ptr(), C.cast(s2, _vp),
+                                              *geom[1:], window_size, C.cast(t, _vp), _p(coef), ws.data_ptr(), nb,
+                                              dev, st))
+        return ws
+
+    def ssim_finalize(self, img1, window_size, size_average, ws, acc, value, reduce=True):
+        """acc fp64 / value fp32: {sum, count} / [1] (size_average), else [N] (2-D) or [N][W'] (3-D); reduce=False
+        recomputes value from acc only"""
+        dev, st = self._ds(acc)
+        geom, _ = self._ssim_geom(img1)
+        self._check(self.lib.b200seg_ssim_finalize(*geom, window_size, int(bool(size_average)), int(bool(reduce)),
+                                                   ws.data_ptr(), ws.numel() * 8, acc.data_ptr(), value.data_ptr(),
+                                                   dev, st))
+
+    def ssim_bwd(self, img1, img2, window_size, taps, coef, size_average, gout, acc, grad1, grad2):
+        """grad1 / grad2: fp32 contiguous in the images' shape, or None"""
+        dev, st = self._ds(img1)
+        geom, s1 = self._ssim_geom(img1)
+        _, s2 = self._ssim_geom(img2)
+        t = (C.c_float * window_size)(*[float(v) for v in taps])
+        self._check(self.lib.b200seg_ssim_bwd(geom[0], img1.data_ptr(), C.cast(s1, _vp), img2.data_ptr(), C.cast(s2, _vp),
+                                              *geom[1:], window_size, C.cast(t, _vp), coef.data_ptr(),
+                                              int(bool(size_average)), gout.data_ptr(), acc.data_ptr(), _p(grad1),
+                                              _p(grad2), dev, st))
 
     # ------------------------------------------------------------------ per-step accuracy (model/metric.py)
     def metric_partials(self, probs, labels, threshold, metric):

@@ -142,6 +142,15 @@ int segmetric3d_points(const void* real, int rdt, const void* pred, int pdt, int
                        const double* spacing, void* ws, long long ws_bytes, long long cap_r, long long cap_p,
                        long long* real_idx, long long* pred_idx, double* real_nn, double* pred_nn, int device,
                        cudaStream_t s);
+int64_t ssim_workspace(int dims, int N, int C, int D, int H, int W, int k);
+int ssim_fwd(int dims, const float* x, const int64_t* xs, const float* y, const int64_t* ys, int N, int C, int D,
+             int H, int W, int k, const float* taps, double* coef, void* ws, long long ws_bytes, int device,
+             cudaStream_t st);
+int ssim_finalize(int dims, int N, int C, int D, int H, int W, int k, int size_average, int reduce, const void* ws,
+                  long long ws_bytes, double* acc, float* value, cudaStream_t st);
+int ssim_bwd(int dims, const float* x, const int64_t* xs, const float* y, const int64_t* ys, int N, int C, int D,
+             int H, int W, int k, const float* taps, const double* coef, int size_average, const float* gout,
+             const double* acc, float* dx, float* dy, int device, cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -676,6 +685,42 @@ int b200seg_segmetric3d_points(const void* real, int real_dtype, const void* pre
   return segmetric3d_points(real, real_dtype, pred, pred_dtype, N, D, H, W, spacing_zyx, workspace, workspace_bytes,
                             cap_r, cap_p, reinterpret_cast<long long*>(real_idx),
                             reinterpret_cast<long long*>(pred_idx), real2pred, pred2real, device, ST(stream));
+}
+
+int64_t b200seg_ssim_workspace(int dims, int N, int C, int D, int H, int W, int window_size) {
+  if ((dims != 2 && dims != 3) || N < 1 || C < 1 || H < 1 || W < 1 || (dims == 3 && D < 1) || window_size < 1 ||
+      window_size > 31)
+    return 0;
+  return ssim_workspace(dims, N, C, D, H, W, window_size);
+}
+
+int b200seg_ssim_fwd(int dims, const float* img1, const int64_t* strides1, const float* img2, const int64_t* strides2,
+                     int N, int C, int D, int H, int W, int window_size, const float* taps, double* coef,
+                     void* workspace, int64_t workspace_bytes, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(img1 && img2 && strides1 && strides2, "b200seg_ssim_fwd: null argument");
+  B200_DEVICE(device);
+  return ssim_fwd(dims, img1, strides1, img2, strides2, N, C, D, H, W, window_size, taps, coef, workspace,
+                  workspace_bytes, device, ST(stream));
+}
+
+int b200seg_ssim_finalize(int dims, int N, int C, int D, int H, int W, int window_size, int size_average, int reduce,
+                          const void* workspace, int64_t workspace_bytes, double* acc, float* value, int device,
+                          b200seg_stream stream) {
+  B200_CHECK_ARG(acc && value, "b200seg_ssim_finalize: null argument");
+  B200_DEVICE(device);
+  return ssim_finalize(dims, N, C, D, H, W, window_size, size_average, reduce, workspace, workspace_bytes, acc, value,
+                       ST(stream));
+}
+
+int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const float* img2, const int64_t* strides2,
+                     int N, int C, int D, int H, int W, int window_size, const float* taps, const double* coef,
+                     int size_average, const float* gout, const double* acc, float* grad1, float* grad2, int device,
+                     b200seg_stream stream) {
+  B200_CHECK_ARG(img1 && img2 && strides1 && strides2 && coef && gout, "b200seg_ssim_bwd: null argument");
+  B200_CHECK_ARG(grad1 || grad2, "b200seg_ssim_bwd: no gradient requested");
+  B200_DEVICE(device);
+  return ssim_bwd(dims, img1, strides1, img2, strides2, N, C, D, H, W, window_size, taps, coef, size_average, gout,
+                  acc, grad1, grad2, device, ST(stream));
 }
 
 }  // extern "C"

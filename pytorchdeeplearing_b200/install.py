@@ -3,7 +3,7 @@
 The reference wrappers bind the classes at import time (``from networks.VNet3d import VNet3d``
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
 rebinds those names in whichever of ``networks``, ``networks.*``, ``model.modelVNet``,
-``model.modelUnet``, ``model.losses``, ``model.metric`` are already imported (and in ``sys.modules`` entries
+``model.modelUnet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM`` are already imported (and in ``sys.modules`` entries
 imported later via the same names).  ``uninstall`` restores the originals.
 """
 from __future__ import annotations
@@ -19,16 +19,20 @@ _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "B
 # the further model/losses.py classes (bound there, not imported by the wrappers)
 _EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss", "MutilELDiceLoss",
                    "LovaszLoss")
+# model/lossesSSIM.py
+_SSIM_NAMES = ("SSIM", "SSIM3D", "ssim", "ssim3D")
 _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet2d", "model",
-            "model.losses", "model.metric", "model.modelVNet", "model.modelUnet")
+            "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM")
 
 
 def install() -> int:
     """Rebind the reference's names to the drop-in implementations. Returns the number of bindings changed."""
     from . import networks as nets, losses, metric
+    from .ssim import SSIM, SSIM3D, ssim, ssim3D       # the package's ``ssim`` attribute is the function, not the module
     table = {n: getattr(nets, n) for n in _NET_NAMES}
     table.update({n: getattr(losses, n) for n in _LOSS_NAMES + _EXT_LOSS_NAMES})
     table.update({n: getattr(metric, n) for n in _METRIC_NAMES})     # per-step accuracy, model/modelVNet.py:582
+    table.update(zip(_SSIM_NAMES, (SSIM, SSIM3D, ssim, ssim3D)))
     count = 0
     for modname in _MODULES:
         mod = sys.modules.get(modname)
