@@ -382,6 +382,21 @@ int b200seg_head_mask(const b200seg_tensor* x, const float* w, const float* bias
 int b200seg_mask_logits(const float* logits, int64_t nvox, int C, float threshold, uint8_t* mask, int device,
                         b200seg_stream stream);
 
+/* ---- classifier head of ResNet2d / ResNet3d (networks/ResNet3d.py:61-118): GlobalAveragePooling -> Linear(C, Hd)
+ * -> ReLU -> Linear(Hd, K).  x: the last encoder activation (N, D, H, W, C), F32 or BF16, with channel pitch.
+ * w1 [Hd][C], b1 [Hd], w2 [K][Hd], b2 [K]: fp32 in nn.Linear layout.  C, Hd, K in [1, 1024].  Two launches each way,
+ * fixed-order sums without atomics (reruns are bit-identical), no allocation, no host synchronisation.
+ *   fwd: pooled [N][C] = mean over voxels, hidden [N][Hd] = relu(w1 pooled + b1), logits [N][K] = w2 hidden + b2 (fp32)
+ *   bwd: dlogits [N][K] -> dw1, db1, dw2, db2 (written, not accumulated) and the dense activation gradient
+ *        dx (N, D, H, W, C) = (w1^T ((w2^T dlogits) * [hidden > 0])) / (D*H*W) broadcast over the voxels (dx's dtype);
+ *        work: fp32 scratch of N*(Hd + C) elements. */
+int b200seg_cls_head_fwd(const b200seg_tensor* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                         int hidden_width, int ncls, float* pooled, float* hidden, float* logits, int device,
+                         b200seg_stream stream);
+int b200seg_cls_head_bwd(const float* dlogits, const float* pooled, const float* hidden, const float* w1,
+                         const float* w2, int hidden_width, int ncls, float* work, const b200seg_tensor* dx, float* dw1,
+                         float* db1, float* dw2, float* db2, int device, b200seg_stream stream);
+
 /* ---- device-side input staging (SURVEY.md 8f-4): the per-sample host work of the reference's datasets, from the raw
  * 8-bit images.  datasetModelSegwithopencv.__getitem__ (model/dataset.py:138-142): image = (image - image.mean()) /
  * image.std() in float64 with the population std, then .float(); labels .long() (dataset.py:150-157) with the trainer's

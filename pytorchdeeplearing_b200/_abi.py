@@ -109,6 +109,8 @@ _SIGNATURES = {
     "b200seg_dropout_masks": ([_vp, _vp, _i, _i, C.c_double, _vp, _i, _vp], C.c_int),
     "b200seg_head_mask": ([_PT, _vp, _vp, _vp, _i, _f, _i, _vp], C.c_int),
     "b200seg_mask_logits": ([_vp, _i64, _i, _f, _vp, _i, _vp], C.c_int),
+    "b200seg_cls_head_fwd": ([_PT, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_cls_head_bwd": ([_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _PT, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_stage_u8_sums": ([_vp, _i, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_stage_u8_normalize": ([_vp, _i, _i64, _vp, _vp, _i, _i, _vp], C.c_int),
     "b200seg_stage_labels_u8": ([_vp, _i64, _i, _vp, _i, _vp], C.c_int),
@@ -540,6 +542,25 @@ class CudaBackend:
         self._check(self.lib.b200seg_head_bwd(C.byref(d1), dlogits.data_ptr(), w.data_ptr(), C.byref(d2),
                                               dw.data_ptr(), db.data_ptr(), nc, dev, st))
         return True
+
+    def cls_head_fwd(self, x, w1, b1, w2, b2, pooled, hidden, logits):
+        """classifier head (ResNet2d / ResNet3d): x (N,D,H,W,C) -> pooled [N][C], hidden [N][Hd], logits [N][K] fp32;
+        w1/b1/w2/b2 the nn.Linear parameters"""
+        dev, st = self._ds(x)
+        dx = _desc(x)
+        self._check(self.lib.b200seg_cls_head_fwd(C.byref(dx), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
+                                                  b2.data_ptr(), w1.shape[0], w2.shape[0], pooled.data_ptr(),
+                                                  hidden.data_ptr(), logits.data_ptr(), dev, st))
+
+    def cls_head_bwd(self, dlogits, pooled, hidden, w1, w2, work, dx, dw1, db1, dw2, db2):
+        """d logits [N][K] -> dw1, db1, dw2, db2 (written) and dx (N,D,H,W,C) = the broadcast pooled gradient;
+        work: fp32 scratch of N*(Hd + C) elements"""
+        dev, st = self._ds(dlogits)
+        d = _desc(dx)
+        self._check(self.lib.b200seg_cls_head_bwd(dlogits.data_ptr(), pooled.data_ptr(), hidden.data_ptr(),
+                                                  w1.data_ptr(), w2.data_ptr(), w1.shape[0], w2.shape[0],
+                                                  work.data_ptr(), C.byref(d), dw1.data_ptr(), db1.data_ptr(),
+                                                  dw2.data_ptr(), db2.data_ptr(), dev, st))
 
     @staticmethod
     def _label_dtype(labels):

@@ -151,6 +151,11 @@ int ssim_finalize(int dims, int N, int C, int D, int H, int W, int k, int size_a
 int ssim_bwd(int dims, const float* x, const int64_t* xs, const float* y, const int64_t* ys, int N, int C, int D,
              int H, int W, int k, const float* taps, const double* coef, int size_average, const float* gout,
              const double* acc, float* dx, float* dy, int device, cudaStream_t st);
+int cls_head_fwd(const b200seg_tensor* x, const float* w1, const float* b1, const float* w2, const float* b2, int Hd,
+                 int K, float* pooled, float* hidden, float* logits, cudaStream_t st);
+int cls_head_bwd(const float* dlogits, const float* pooled, const float* hidden, const float* w1, const float* w2,
+                 int Hd, int K, float* work, const b200seg_tensor* dx, float* dw1, float* db1, float* dw2, float* db2,
+                 int device, cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -563,6 +568,28 @@ int b200seg_mask_logits(const float* logits, int64_t nvox_, int C, float thresho
   B200_CHECK_ARG(logits && mask && nvox_ > 0 && C > 0, "b200seg_mask_logits: bad argument");
   B200_DEVICE(device);
   return mask_logits(logits, nvox_, C, threshold, mask, device, ST(stream));
+}
+
+int b200seg_cls_head_fwd(const b200seg_tensor* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                         int hidden_width, int ncls, float* pooled, float* hidden, float* logits, int device,
+                         b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  B200_CHECK_ARG(w1 && b1 && w2 && b2 && pooled && hidden && logits, "b200seg_cls_head_fwd: null argument");
+  B200_CHECK_ARG(x->n <= 65535, "b200seg_cls_head_fwd: batch must be at most 65535 (got %d)", x->n);
+  B200_DEVICE(device);
+  return cls_head_fwd(x, w1, b1, w2, b2, hidden_width, ncls, pooled, hidden, logits, ST(stream));
+}
+
+int b200seg_cls_head_bwd(const float* dlogits, const float* pooled, const float* hidden, const float* w1,
+                         const float* w2, int hidden_width, int ncls, float* work, const b200seg_tensor* dx, float* dw1,
+                         float* db1, float* dw2, float* db2, int device, b200seg_stream stream) {
+  REQ_TENSOR(dx, "dx");
+  B200_CHECK_ARG(dlogits && pooled && hidden && w1 && w2 && work && dw1 && db1 && dw2 && db2,
+                 "b200seg_cls_head_bwd: null argument");
+  B200_CHECK_ARG(dx->n <= 65535, "b200seg_cls_head_bwd: batch must be at most 65535 (got %d)", dx->n);
+  B200_DEVICE(device);
+  return cls_head_bwd(dlogits, pooled, hidden, w1, w2, hidden_width, ncls, work, dx, dw1, db1, dw2, db2, device,
+                      ST(stream));
 }
 
 int b200seg_stage_u8_sums(const uint8_t* img, int n, int64_t per_sample, uint64_t* sums, int device,

@@ -1,6 +1,6 @@
 """Layer program of the segmentation hot path (host side, Python).
 
-The engine turns one forward/backward of ``VNet3d`` / ``UNet3d`` / ``UNet2d`` into a sequence
+The engine turns one forward/backward of ``VNet3d`` / ``UNet3d`` / ``UNet2d`` / ``ResNet3d`` into a sequence
 of calls on a *backend* whose methods map 1:1 onto the ``extern "C"`` entry points of
 ``include/b200seg.h`` (``_abi.CudaBackend``).  It owns no arithmetic: every FLOP and every
 byte moved happens inside a backend op (= one hand-written sm_90a kernel launch).
@@ -331,15 +331,16 @@ class Engine:
             self._launch_deferred()                    # behind the first convolution of the pass
 
     def conv_gn(self, kind: int, wname: str, bname: Optional[str], gname: str, x: Tensor,
-                out_sp: Sequence[int], cout: int) -> Layer:
-        """conv + stats + finalize.  The activation itself is produced later by ``apply``."""
+                out_sp: Sequence[int], cout: int, drop: bool = True) -> Layer:
+        """conv + stats + finalize.  The activation itself is produced later by ``apply``.  ``drop=False``: a layer
+        without Dropout (it takes no mask from the pass's list)."""
         L = Layer(kind, wname, bname, gname, x=x)
         self._tag(wname)
         n = x.shape[0]
         L.y = self.new(x, out_sp, cout)
         stats = self.zeros((n, cout, 2), torch.float64, x.device)
         self.conv_raw(kind, wname, bname, x, L.y, stats)
-        L.scale = self._next_mask()
+        L.scale = self._next_mask() if drop else None
         vox = 1
         for s in out_sp:
             vox *= s
@@ -638,6 +639,107 @@ class Engine:
         return flat
 
     vnet3d_backward = vnet_backward
+
+    # ================================================================== ResNet3d / ResNet2d
+    def resnet_forward(self, P: Dict[str, Tensor], x: Tensor, masks: Optional[List[Tensor]],
+                       need_grad: bool) -> Tensor:
+        """ResNet3d.forward / ResNet2d.forward (reference networks/ResNet3d.py:98-118, ResNet2d.py:99-119): the VNet
+        encoder with Dropout only in the four DownTransitions, then GlobalAveragePooling -> Linear -> ReLU -> Linear.
+        ``do1`` (ResNet3d.py:51-55) drops ``down`` in place, so the residual adds the dropped tensor too: the same
+        algebra as the VNet down block.  ``x``: (N,Cin,[D,]H,W) fp32.  Returns (N, numclass) fp32 logits."""
+        self.P, self.masks, self._mi, self.layers, self.need_grad = P, masks, 0, [], need_grad
+        sv = self.saved = {}
+        dims = self.dims
+        n, cin = x.shape[0], x.shape[1]
+        self._begin_pass(n, x.device, backward=False)
+        if dims == 3:
+            sp0 = tuple(x.shape[2:])
+            xin = x.permute(0, 2, 3, 4, 1)
+        else:
+            sp0 = (1,) + tuple(x.shape[2:])
+            xin = x.permute(0, 2, 3, 1).unsqueeze(1)
+        if cin != 1:
+            xin = xin.contiguous()
+        f = P["in_tr.conv1.weight"].shape[0]
+        sps = [sp0]
+        for _ in range(4):
+            s_ = sps[-1]
+            sps.append((s_[0] // 2 if dims == 3 else 1, s_[1] // 2, s_[2] // 2))
+        ch = [f, 2 * f, 4 * f, 8 * f, 16 * f]
+        vox = [sp[0] * sp[1] * sp[2] for sp in sps]
+        nconvs = (("down_tr32", 2), ("down_tr64", 3), ("down_tr128", 3), ("down_tr256", 3))
+        specs = [("in_tr.conv1.weight", K3, vox[0], vox[0], False), ("in_tr.conv2.weight", K1, vox[0], vox[0], False)]
+        for i, (name, nops) in enumerate(nconvs):
+            specs.append((name + ".down_conv.weight", DOWN, vox[i + 1], vox[i], True))
+            specs += [(f"{name}.ops.{j}.conv1.weight", K3, vox[i + 1], vox[i + 1], True) for j in range(nops)]
+        self._batch, self._ov = n, overlap_mask("resnet", dims)
+        self._prepack(specs, need_grad, n_early=5)         # in_tr (2) + down_tr32 (down conv + 2 ops)
+
+        # ---- InputTransition3d (ResNet3d.py:24-41): one bn1 for both branches, no dropout
+        La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f, drop=False)
+        Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f, drop=False)
+        out = self.act(La, self.new(x, sp0, f), L2=Lb)
+        sv["in_tr"] = (La, Lb)
+
+        # ---- DownTransition3d x4 (ResNet3d.py:44-58): the LUConv stacks have no dropout
+        for i, (name, nops) in enumerate(nconvs):
+            co, sp = ch[i + 1], sps[i + 1]
+            Ld = self.conv_gn(DOWN, name + ".down_conv.weight", name + ".down_conv.bias", name + ".bn1", out, sp, co)
+            down = self.act(Ld, self.new(x, sp, co))
+            h, ops = down, []
+            for j in range(nops):
+                Lo = self.conv_gn(K3, f"{name}.ops.{j}.conv1.weight", f"{name}.ops.{j}.conv1.bias",
+                                  f"{name}.ops.{j}.bn1", h, sp, co, drop=False)
+                ops.append(Lo)
+                h = self.act(Lo, self.new(x, sp, co), res=down if j == nops - 1 else None)   # ResNet3d.py:57
+            sv[name] = (Ld, ops)
+            out = h
+
+        # ---- GlobalAveragePooling + fc_layers (ResNet3d.py:61-69,93-96)
+        self._tag("fc_layers")
+        if self._deferred is not None:
+            self._launch_deferred()
+        self._join_fwd_side()                      # the last forward op: nothing of this pass stays un-joined
+        w1, w2 = P["fc_layers.0.weight"], P["fc_layers.2.weight"]
+        pooled = torch.empty((n, out.shape[-1]), dtype=torch.float32, device=x.device)
+        hidden = torch.empty((n, w1.shape[0]), dtype=torch.float32, device=x.device)
+        logits = torch.empty((n, w2.shape[0]), dtype=torch.float32, device=x.device)
+        self.be.cls_head_fwd(out, w1, P["fc_layers.0.bias"], w2, P["fc_layers.2.bias"], pooled, hidden, logits)
+        sv["head"] = (out, pooled, hidden)
+        return logits
+
+    def resnet_backward(self, g_logits: Tensor) -> Tensor:
+        """Gradients of all 70 parameters given d loss / d logits ((N, numclass) fp32, contiguous).  Returns the flat
+        fp32 bucket; ``self.grads`` holds the views."""
+        sv = self.saved
+        dev = g_logits.device
+        flat = self.alloc_grads(dev)
+        n = g_logits.shape[0]
+        self._begin_pass(n, dev, backward=True)
+        out, pooled, hidden = sv["head"]
+        self._tag("fc_layers")
+        w1, w2 = self.P["fc_layers.0.weight"], self.P["fc_layers.2.weight"]
+        g = torch.empty(out.shape, dtype=self.T, device=dev)
+        work = torch.empty(n * (w1.shape[0] + w1.shape[1]), dtype=torch.float32, device=dev)
+        gv = self._grad_view
+        self.be.cls_head_bwd(g_logits, pooled, hidden, w1, w2, work, g, gv("fc_layers.0.weight"),
+                             gv("fc_layers.0.bias"), gv("fc_layers.2.weight"), gv("fc_layers.2.bias"))
+        for i, name in zip((3, 2, 1, 0), ["down_tr256", "down_tr128", "down_tr64", "down_tr32"]):
+            Ld, ops = sv[name]
+            g_out = g                                    # d/d(out) ; out = ops(down) + down
+            gh = g_out
+            for j in reversed(range(len(ops))):
+                gh = self.bwd_layer(ops[j], gh, True, dx_addend=g_out if j == 0 else None,
+                                    prev=ops[j - 1] if j > 0 else Ld)
+            g = self.bwd_layer(Ld, gh, True)
+            if i == 3:
+                self._flush_bucket("down_tr256.down_conv.weight")
+                self._early_unpack()
+        La, Lb = sv["in_tr"]
+        self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
+        self.bwd_layer(Lb, g, False)
+        self._finish_backward()
+        return flat
 
     # ================================================================== UNet3d / UNet2d
     def unet_forward(self, P: Dict[str, Tensor], x: Tensor, masks: Optional[List[Tensor]],

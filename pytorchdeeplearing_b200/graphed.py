@@ -102,9 +102,16 @@ class GraphedStep:
         P = dict(zip(m._pnames, [p.detach() for _, p in m.named_parameters()]))
         masks = self._masks() if m.training else None
         x = self.x if self.x.dtype == torch.float32 else self.x.float()
-        logits, probs = getattr(eng, m._arch + "_forward")(P, x, masks, True)
-        perm = (0, 2, 3, 4, 1) if logits.dim() == 5 else (0, 2, 3, 1)
-        z = logits.permute(*perm)
+        out = getattr(eng, m._arch + "_forward")(P, x, masks, True)
+        self._cls = isinstance(out, torch.Tensor)
+        if self._cls:
+            # classifier: (N, C) logits, a volume of one voxel per sample for the loss kernels (losses.prepare_logits)
+            logits, probs = out, None
+            z = logits.view(logits.shape[0], 1, 1, 1, logits.shape[1])
+        else:
+            logits, probs = out
+            perm = (0, 2, 3, 4, 1) if logits.dim() == 5 else (0, 2, 3, 1)
+            z = logits.permute(*perm)
         if not z.is_contiguous():
             z = z.contiguous()
         c, n = z.shape[-1], z.shape[0]
@@ -151,7 +158,10 @@ class GraphedStep:
                 be.loss_bwd_ss(z, self.y, lcoef, self._one, dz)
             else:
                 be.loss_bwd(z, self.y, lcoef, self._one, dz)
-        g = dz if dz.dim() == 5 else dz.unsqueeze(1)
+        if self._cls:
+            g = dz.view(dz.shape[0], c)
+        else:
+            g = dz if dz.dim() == 5 else dz.unsqueeze(1)
         self._split_off = None
         eng.bucket_hook = self._bucket_ready if self.dp else None
         flat = getattr(eng, self.model._arch + "_backward")(g)

@@ -17,10 +17,18 @@ from . import runtime
 from .engine import Engine
 
 
+def _require_segmenter(model) -> None:
+    if getattr(model, "_arch", None) == "resnet":
+        raise TypeError(f"{type(model).__name__} is a classifier: it has no segmentation mask to predict; call the "
+                        "model itself for its (N, numclass) logits, as the reference's ResNet predict does")
+
+
 @torch.no_grad()
 def predict_mask(model, x: torch.Tensor, out_threshold: float = 0.5) -> torch.Tensor:
     """x (N, Cin, [D,] H, W) on the model's device -> uint8 mask (N, [D,] H, W): ``(sigmoid > out_threshold) * 255``
-    for a one-class head, ``argmax`` over the classes otherwise (model/modelVNet.py:668-675).  Eval-mode forward."""
+    for a one-class head, ``argmax`` over the classes otherwise (model/modelVNet.py:668-675).  Eval-mode forward.
+    Segmentation nets only: a classifier (ResNet2d / ResNet3d) raises ``TypeError``."""
+    _require_segmenter(model)
     be = runtime.get_backend(x)
     eng = Engine(be, runtime.act_dtype(), model._dims)
     eng.mask_threshold = float(out_threshold)
@@ -35,6 +43,7 @@ def predict_mask(model, x: torch.Tensor, out_threshold: float = 0.5) -> torch.Te
 def predict(model, full_img, out_threshold: float = 0.5) -> np.ndarray:
     """``XModel.predict(full_img, out_threshold)`` (model/modelVNet.py:655-676): numpy image (Cin, [D,] H, W) ->
     numpy uint8 mask ([D,] H, W)."""
+    _require_segmenter(model)
     dev = next(model.parameters()).device
     img = torch.as_tensor(np.ascontiguousarray(full_img)).float().unsqueeze(0).to(dev)
     was_training = model.training
@@ -63,6 +72,7 @@ def sliding_window_mask(model, image, patch_size: Sequence[int], step: Sequence[
     (Cin, D, H, W) [or image (Cin, H, W)] with ``patch_size`` windows every ``step`` voxels (default: half a patch, as
     the reference), predict ``batch`` windows per forward on the device, accumulate the masks on the device and
     binarise the union (``out_mask[out_mask != 0] = 1``).  Only the final uint8 volume is copied to the host."""
+    _require_segmenter(model)
     dev = next(model.parameters()).device
     vol = torch.as_tensor(np.ascontiguousarray(image)).float().to(dev)
     dims = model._dims

@@ -3,7 +3,7 @@
 The reference wrappers bind the classes at import time (``from networks.VNet3d import VNet3d``
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
 rebinds those names in whichever of ``networks``, ``networks.*``, ``model.modelVNet``,
-``model.modelUnet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM`` are already imported (and in ``sys.modules`` entries
+``model.modelUnet``, ``model.modelResNet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM`` are already imported (and in ``sys.modules`` entries
 imported later via the same names).  ``uninstall`` restores the originals.
 """
 from __future__ import annotations
@@ -12,7 +12,7 @@ import sys
 
 _SAVED = []
 
-_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet2d")
+_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet2d", "ResNet2d", "ResNet3d")
 _METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "Seg_Metirc3d")
 _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
@@ -22,7 +22,8 @@ _EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "Bin
 # model/lossesSSIM.py
 _SSIM_NAMES = ("SSIM", "SSIM3D", "ssim", "ssim3D")
 _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet2d", "model",
-            "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM")
+            "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
+            "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet")
 
 
 def install() -> int:

@@ -27,10 +27,16 @@ def _check_labels_default() -> bool:
 
 
 def prepare_logits(logits: torch.Tensor):
-    """channels-last fp32 view (N, ..., C) of NCDHW / NCHW logits (free when they come from the drop-in networks)"""
+    """channels-last fp32 view (N, ..., C) of NCDHW / NCHW logits (free when they come from the drop-in networks).
+    Classifier logits (N, C) become an (N, 1, 1, 1, C) volume of one voxel per sample, which is what the reference's
+    ``.view(bs, C, -1)`` makes of them (model/losses.py:143,253); ``perm`` is then None."""
     z = logits.detach()
-    perm = (0, 2, 3, 4, 1) if z.dim() == 5 else (0, 2, 3, 1)
-    z = z.permute(*perm)
+    if z.dim() == 2:
+        perm = None
+        z = z.reshape(z.shape[0], 1, 1, 1, z.shape[1])
+    else:
+        perm = (0, 2, 3, 4, 1) if z.dim() == 5 else (0, 2, 3, 1)
+        z = z.permute(*perm)
     if z.dtype != torch.float32:
         z = z.float()                               # losses.py:47 ``.float()``
     if not z.is_contiguous():
@@ -50,6 +56,14 @@ def prepare_labels(labels: torch.Tensor, c: int):
     if not t.is_contiguous():
         t = t.contiguous()
     return t
+
+
+def logits_grad(dz: torch.Tensor, perm):
+    """d loss / d logits in the caller's layout: the inverse of ``prepare_logits``"""
+    if perm is None:
+        return dz.view(dz.shape[0], dz.shape[-1])
+    inv = (0, 4, 1, 2, 3) if dz.dim() == 5 else (0, 3, 1, 2)
+    return dz.permute(*inv)
 
 
 class _FusedLoss(torch.autograd.Function):
@@ -101,8 +115,7 @@ class _FusedLoss(torch.autograd.Function):
             be.loss_bwd_ss(z, t, lcoef, g, dz)
         else:
             be.loss_bwd(z, t, lcoef, g, dz)
-        inv = (0, 4, 1, 2, 3) if z.dim() == 5 else (0, 3, 1, 2)
-        return dz.permute(*inv), None, None, None, None, None, None
+        return logits_grad(dz, ctx.perm), None, None, None, None, None, None
 
 
 def ignore_label(ignore):
@@ -149,6 +162,7 @@ class _LovaszLoss(torch.autograd.Function):
         if owner is not None:
             owner._metric_sums = metric
         ctx.save_for_backward(z, t, coef, scale)
+        ctx.perm = perm
         ctx.per_image = per_image
         return loss
 
@@ -159,8 +173,7 @@ class _LovaszLoss(torch.autograd.Function):
         dz = torch.empty_like(z)
         g = gout.detach().to(torch.float32).reshape(1).contiguous()
         be.lovasz_bwd(z, t, ctx.per_image, coef, scale, g, dz)
-        inv = (0, 4, 1, 2, 3) if z.dim() == 5 else (0, 3, 1, 2)
-        return dz.permute(*inv), None, None, None, None
+        return logits_grad(dz, ctx.perm), None, None, None, None
 
 
 class _LossBase(nn.Module):
@@ -171,7 +184,8 @@ class _LossBase(nn.Module):
 
     def last_metric(self) -> torch.Tensor:
         """fp32 [2] = (dice, iou) of the last forward: ``dice_coeff(probs, y)`` for one class,
-        ``multiclass_dice_coeff(probs, y)`` otherwise -- without reading ``probs``."""
+        ``multiclass_dice_coeff(probs, y)`` otherwise -- without reading ``probs``.  On classifier logits (N, C) it
+        is the same Dice / IoU formula over one voxel per sample, not a classification accuracy."""
         if self._metric_sums is None:
             raise RuntimeError("no forward has run yet")
         be = runtime.get_backend(self._metric_sums)

@@ -5,6 +5,8 @@ from .Unet2d import UNet2d
 from .Unet3d import UNet3d
 from .VNet3d import VNet3d
 from .VNet2d import VNet2d
+from .ResNet2d import ResNet2d
+from .ResNet3d import ResNet3d
 
 
 def initialize_weights(net):
@@ -25,4 +27,4 @@ def initialize_weights(net):
         nn.init.constant_(net.bias.data, 0)
 
 
-__all__ = ["UNet2d", "UNet3d", "VNet3d", "VNet2d", "initialize_weights"]
+__all__ = ["UNet2d", "UNet3d", "VNet3d", "VNet2d", "ResNet2d", "ResNet3d", "initialize_weights"]

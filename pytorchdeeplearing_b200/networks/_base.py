@@ -45,33 +45,69 @@ class _SegNetFunction(torch.autograd.Function):
         if g_logits is None:
             return (None, None, None, None) + (None,) * len(ctx.names)
         g = g_logits.permute(0, 2, 3, 4, 1) if g_logits.dim() == 5 else g_logits.permute(0, 2, 3, 1).unsqueeze(1)
-        if not g.is_contiguous():
-            g = g.contiguous()
-        if g.dtype != torch.float32:
-            g = g.float()
-        enabled, group = runtime.dp_state()
-        works, split = [], [None]
-        if enabled:
-            import torch.distributed as dist
+        return _net_backward(ctx, eng, g)
 
-            def bucket_ready(flat_, off):
-                # gradients flat[off:] (deepest encoder block .. head, ~96 % of the bytes) are final: their SUM
-                # all-reduce starts now and overlaps the rest of backward (SURVEY.md section 8e, C1)
-                split[0] = off
-                works.append(dist.all_reduce(flat_[off:], op=dist.ReduceOp.SUM, group=group, async_op=True))
-            eng.bucket_hook = bucket_ready
-        flat = getattr(eng, ctx.arch + "_backward")(g)
-        if enabled:
-            if split[0] is None:
-                dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
-            else:
-                if split[0] > 0:
-                    dist.all_reduce(flat[:split[0]], op=dist.ReduceOp.SUM, group=group)
-                for w in works:
-                    w.wait()
-        grads = [eng.grads[n] for n in ctx.names]
-        ctx.eng = None
-        return (None, None, None, None) + tuple(grads)
+
+def _net_backward(ctx, eng: Engine, g: torch.Tensor):
+    """the engine's backward from d loss / d logits ``g`` (channels-last, or (N, numclass) for a classifier), with the
+    gradient all-reduce of data-parallel runs; returns the autograd tuple of (mod, need_grad, x, masks, *params)"""
+    if not g.is_contiguous():
+        g = g.contiguous()
+    if g.dtype != torch.float32:
+        g = g.float()
+    enabled, group = runtime.dp_state()
+    works, split = [], [None]
+    if enabled:
+        import torch.distributed as dist
+
+        def bucket_ready(flat_, off):
+            # gradients flat[off:] (deepest encoder block .. head, ~96 % of the bytes) are final: their SUM
+            # all-reduce starts now and overlaps the rest of backward (SURVEY.md section 8e, C1)
+            split[0] = off
+            works.append(dist.all_reduce(flat_[off:], op=dist.ReduceOp.SUM, group=group, async_op=True))
+        eng.bucket_hook = bucket_ready
+    flat = getattr(eng, ctx.arch + "_backward")(g)
+    if enabled:
+        if split[0] is None:
+            dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
+        else:
+            if split[0] > 0:
+                dist.all_reduce(flat[:split[0]], op=dist.ReduceOp.SUM, group=group)
+            for w in works:
+                w.wait()
+    grads = [eng.grads[n] for n in ctx.names]
+    ctx.eng = None
+    return (None, None, None, None) + tuple(grads)
+
+
+class _ClsNetFunction(torch.autograd.Function):
+    """Single-output form for the classifiers (ResNet2d / ResNet3d): forward (x, *params) -> (N, numclass) logits;
+    backward: d logits -> d params."""
+
+    @staticmethod
+    def forward(ctx, mod, need_grad, x, masks, *params):
+        be = runtime.get_backend(x)
+        eng = Engine(be, runtime.act_dtype(), mod._dims)
+        P = dict(zip(mod._pnames, [p.detach() for p in params]))
+        xx = x.detach()
+        if xx.dtype != torch.float32:
+            xx = xx.float()
+        logits = getattr(eng, mod._arch + "_forward")(P, xx, masks, need_grad)
+        ctx.eng = eng if need_grad else None
+        ctx.arch = mod._arch
+        ctx.names = mod._pnames
+        ctx.set_materialize_grads(False)
+        return logits
+
+    @staticmethod
+    def backward(ctx, g_logits):
+        eng: Engine = ctx.eng
+        if eng is None:
+            raise RuntimeError("pytorchdeeplearing_b200: backward through the network a second time (the saved "
+                               "activations are released after the first backward; retain_graph is not supported)")
+        if g_logits is None:
+            return (None, None, None, None) + (None,) * len(ctx.names)
+        return _net_backward(ctx, eng, g_logits)
 
 
 class MaskPlan:
@@ -117,6 +153,7 @@ class SegNetBase(nn.Module):
 
     _arch = ""
     _dims = 3
+    _function = _SegNetFunction       # (logits, probs); the classifiers return logits only (_ClsNetFunction)
     dropout_masks: Optional[List[torch.Tensor]] = None     # test hook: inject (N,C) scales
 
     def _finish_init(self):
@@ -183,7 +220,7 @@ class SegNetBase(nn.Module):
         masks = self._draw_masks(x)
         # (grad mode is always off inside Function.forward, so the decision is taken here)
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-        return _SegNetFunction.apply(self, need_grad, x, masks, *params)
+        return self._function.apply(self, need_grad, x, masks, *params)
 
 
 class _Holder(nn.Module):
