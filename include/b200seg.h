@@ -226,6 +226,33 @@ int b200seg_gn_bwd_apply(const b200seg_tensor* g, const b200seg_tensor* y, const
 /* out[c] = sum_{n,d,h,w} dy[...,c]   (bias gradient of convs without GroupNorm) */
 int b200seg_colsum(const b200seg_tensor* dy, float* out, int device, b200seg_stream stream);
 
+/* ---- fused input block (VNet3d.py:25-43 / ResNet3d.py:24-41): conv1 3x3x3 and conv2 1x1x1 of a one-channel fp32
+ * image x, 16 channels each, ONE GroupNorm(8, 16) applied to each branch with its own statistics, dropout, ReLU and
+ * the sum of the branches.  No pass stores the raw stem outputs: each recomputes them from x with the arithmetic of
+ * b200seg_conv's stem kernels, so the results equal b200seg_conv (stats) -> b200seg_apply_gn(y_a, y_b) on the
+ * forward side and b200seg_gn_bwd_reduce_gn -> b200seg_gn_bwd_apply_gn -> b200seg_wgrad per branch on the backward
+ * side.  w3 / w1: the bf16 forward operands (b200seg_pack_weight, [27][16] / [1][16]); gn3 / gn1: the GroupNorm
+ * reference of each branch (8 groups, vox = D*H*W); stats [N][16][2], sums [N][16][3] fp64, zero on entry where
+ * written.  Ask b200seg_stem_gn_supported first (3-D, fp32 x, H % 8 == 0, W a multiple of 16, 16 channels). */
+int b200seg_stem_gn_supported(const b200seg_tensor* x, int cout, int dims);
+/* per-(n, c) sum y, sum y^2 of both branches (what b200seg_conv writes into its stats argument) */
+int b200seg_stem_gn_stats(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                          double* stats3, double* stats1, int device, b200seg_stream stream);
+/* out = relu(y3*A3+B3) + relu(y1*A1+B1); out: bf16, 16 channels, any pitch */
+int b200seg_stem_gn_apply(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                          const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* out, int device,
+                          b200seg_stream stream);
+/* sums3 / sums1 [N][16][3] += {sum g*m, sum g*m*y, sum y} of each branch (b200seg_gn_bwd_reduce_gn's layout) */
+int b200seg_stem_gn_bwd_sums(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                             const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* g, double* sums3,
+                             double* sums1, int device, b200seg_stream stream);
+/* dw3 [27][16] +=, dw1 [16] +=, dgamma, dbeta [16] += (both branches), db3, db1 [16] += (may be NULL): the weight
+ * gradients of both stems with the GroupNorm backward folded in; dy itself never leaves the chip */
+int b200seg_stem_gn_bwd(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                        const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* g, const double* sums3,
+                        const double* sums1, float* dw3, float* dw1, float* dgamma, float* dbeta, float* db3,
+                        float* db1, int device, b200seg_stream stream);
+
 /* ---- nn.MaxPool3d/2d(2,2) (Unet3d.py:18-24) */
 int b200seg_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dims, int device, b200seg_stream stream);
 int b200seg_pool_bwd(const b200seg_tensor* x, const b200seg_tensor* g_out, const b200seg_tensor* addend,

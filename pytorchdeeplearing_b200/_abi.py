@@ -82,6 +82,12 @@ _SIGNATURES = {
     "b200seg_pool_bwd": ([_PT, _PT, _PT, _PT, _i, _i, _vp], C.c_int),
     "b200seg_head_probs": ([_vp, _vp, _i64, _i, _i, _vp], C.c_int),
     "b200seg_head_fwd": ([_PT, _vp, _vp, _vp, _vp, _i, _i, _vp], C.c_int),
+    "b200seg_stem_gn_supported": ([_PT, _i, _i], C.c_int),
+    "b200seg_stem_gn_stats": ([_PT, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_stem_gn_apply": ([_PT, _vp, _vp, _vp, _vp, _PG, _PG, _PT, _i, _vp], C.c_int),
+    "b200seg_stem_gn_bwd_sums": ([_PT, _vp, _vp, _vp, _vp, _PG, _PG, _PT, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_stem_gn_bwd": ([_PT, _vp, _vp, _vp, _vp, _PG, _PG, _PT, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp],
+                            C.c_int),
     "b200seg_head_bwd_supported": ([_i, _i], C.c_int),
     "b200seg_head_bwd": ([_PT, _vp, _vp, _PT, _vp, _vp, _i, _i, _vp], C.c_int),
     "b200seg_loss_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _f, _vp, _vp, _i, _vp], C.c_int),
@@ -481,6 +487,49 @@ class CudaBackend:
         self._check(self.lib.b200seg_gn_bwd_fused_gn(C.byref(dg), C.byref(dyy), C.byref(gg), sums.data_ptr(),
                                                      counter.data_ptr(), C.byref(dd), dgamma.data_ptr(),
                                                      dbeta.data_ptr(), _p(dbias), dev, st))
+
+    # ------------------------------------------------------------------ fused input block (csrc/stem_gn.cu)
+    # w3 / w1: the packed forward operands of the two stems (pack_weight(..., "fwd", torch.bfloat16, ...)); the raw
+    # stem outputs are never stored: every call recomputes them from the fp32 image x (N,D,H,W,1)
+    def stem_gn_ok(self, x, cout, dims):
+        """can the fused input-block kernels take this image (3-D, fp32, one channel, 16 output channels)?"""
+        if x.dtype != torch.float32 or x.dim() != 5 or x.shape[-1] != 1:
+            return False
+        return bool(self.lib.b200seg_stem_gn_supported(C.byref(_desc(x)), cout, dims))
+
+    def _stem_operand(self, wpk):
+        if wpk.code != BF16:
+            wpk = self.pack_weight(wpk.src, wpk.kind, wpk.which, torch.bfloat16, wpk.dims, allow_tc=False)
+        return wpk.t.data_ptr()
+
+    def stem_gn_stats(self, x, w3, b3, w1, b1, stats3, stats1):
+        dev, st = self._ds(x)
+        self._check(self.lib.b200seg_stem_gn_stats(C.byref(_desc(x)), self._stem_operand(w3), _p(b3),
+                                                   self._stem_operand(w1), _p(b1), stats3.data_ptr(),
+                                                   stats1.data_ptr(), dev, st))
+
+    def stem_gn_apply(self, x, w3, b3, w1, b1, gn3, gn1, out):
+        dev, st = self._ds(x)
+        g3, g1, do = self._gn(gn3), self._gn(gn1), _desc(out)
+        self._check(self.lib.b200seg_stem_gn_apply(C.byref(_desc(x)), self._stem_operand(w3), _p(b3),
+                                                   self._stem_operand(w1), _p(b1), C.byref(g3), C.byref(g1),
+                                                   C.byref(do), dev, st))
+
+    def stem_gn_bwd_sums(self, x, w3, b3, w1, b1, gn3, gn1, g, sums3, sums1):
+        dev, st = self._ds(x)
+        g3, g1, dg = self._gn(gn3), self._gn(gn1), _desc(g)
+        self._check(self.lib.b200seg_stem_gn_bwd_sums(C.byref(_desc(x)), self._stem_operand(w3), _p(b3),
+                                                      self._stem_operand(w1), _p(b1), C.byref(g3), C.byref(g1),
+                                                      C.byref(dg), sums3.data_ptr(), sums1.data_ptr(), dev, st))
+
+    def stem_gn_bwd(self, x, w3, b3, w1, b1, gn3, gn1, g, sums3, sums1, dw3, dw1, dgamma, dbeta, db3, db1):
+        dev, st = self._ds(x)
+        g3, g1, dg = self._gn(gn3), self._gn(gn1), _desc(g)
+        self._check(self.lib.b200seg_stem_gn_bwd(C.byref(_desc(x)), self._stem_operand(w3), _p(b3),
+                                                 self._stem_operand(w1), _p(b1), C.byref(g3), C.byref(g1),
+                                                 C.byref(dg), sums3.data_ptr(), sums1.data_ptr(), dw3.data_ptr(),
+                                                 dw1.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), _p(db3),
+                                                 _p(db1), dev, st))
 
     def gn_bwd_reduce(self, g, y, coef, sums):
         dev, st = self._ds(y)

@@ -53,6 +53,11 @@ int stem_mma_conv(int kind, int dims, const b200seg_tensor* x, const void* w, co
 int stem_mma_wgrad_supported(int kind, const b200seg_tensor* a, const b200seg_tensor* b);
 int stem_mma_wgrad(int kind, int dims, const b200seg_tensor* a, const b200seg_tensor* b, float* dwp, int device,
                    cudaStream_t st);
+int stem_gn_supported(const b200seg_tensor* x, int cout, int dims);
+int stem_gn(int mode, const b200seg_tensor* x, const void* wa, const float* ba, const void* wb, const float* bb,
+            const b200seg_gn* gna, const b200seg_gn* gnb, double* stats_a, double* stats_b,
+            const b200seg_tensor* out, const b200seg_tensor* gr, double* sums_a, double* sums_b, float* dwa,
+            float* dwb, float* dgamma, float* dbeta, float* dba, float* dbb, int device, cudaStream_t st);
 int stem_conv_supported(int kind, const b200seg_tensor* x, const b200seg_tensor* y, const b200seg_tensor* addend);
 int stem_conv(int kind, int dims, const b200seg_tensor* x, const void* w, int w_dtype, const float* bias,
               const b200seg_tensor* y, double* stats, int device, cudaStream_t st);
@@ -467,6 +472,50 @@ int b200seg_colsum(const b200seg_tensor* dy, float* out, int device, b200seg_str
   B200_CHECK_ARG(out != nullptr && dy->c <= 4096, "b200seg_colsum: bad argument");
   B200_DEVICE(device);
   return ew_colsum(dy, out, device, ST(stream));
+}
+
+int b200seg_stem_gn_supported(const b200seg_tensor* x, int cout, int dims) {
+  if (x == nullptr || !valid_tensor(x)) return 0;
+  return stem_gn_supported(x, cout, dims);
+}
+
+int b200seg_stem_gn_stats(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                          double* stats3, double* stats1, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  B200_DEVICE(device);
+  return stem_gn(0, x, w3, b3, w1, b1, nullptr, nullptr, stats3, stats1, nullptr, nullptr, nullptr, nullptr, nullptr,
+                 nullptr, nullptr, nullptr, nullptr, nullptr, device, ST(stream));
+}
+
+int b200seg_stem_gn_apply(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                          const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* out, int device,
+                          b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(out, "out");
+  B200_DEVICE(device);
+  return stem_gn(1, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, out, nullptr, nullptr, nullptr, nullptr, nullptr,
+                 nullptr, nullptr, nullptr, nullptr, device, ST(stream));
+}
+
+int b200seg_stem_gn_bwd_sums(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                             const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* g, double* sums3,
+                             double* sums1, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(g, "g");
+  B200_DEVICE(device);
+  return stem_gn(2, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, nullptr, g, sums3, sums1, nullptr, nullptr, nullptr,
+                 nullptr, nullptr, nullptr, device, ST(stream));
+}
+
+int b200seg_stem_gn_bwd(const b200seg_tensor* x, const void* w3, const float* b3, const void* w1, const float* b1,
+                        const b200seg_gn* gn3, const b200seg_gn* gn1, const b200seg_tensor* g, const double* sums3,
+                        const double* sums1, float* dw3, float* dw1, float* dgamma, float* dbeta, float* db3,
+                        float* db1, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(g, "g");
+  B200_DEVICE(device);
+  return stem_gn(3, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, nullptr, g, const_cast<double*>(sums3),
+                 const_cast<double*>(sums1), dw3, dw1, dgamma, dbeta, db3, db1, device, ST(stream));
 }
 
 int b200seg_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dims, int device, b200seg_stream stream) {

@@ -49,6 +49,7 @@ class Layer:
     gn: tuple = None                # (stats, gamma, beta, scale, vox, groups, eps): fused-coefficient path
     scale: Optional[Tensor] = None  # (N,Cout) dropout scale or None
     pre_sums: Optional[Tensor] = None   # backward sums already accumulated by the epilogue of the conv that produced g
+    wpk: object = None              # fused input block: packed forward operand of the stem (``y`` is never stored)
 
 
 def _taps(kind: int, dims: int) -> int:
@@ -356,6 +357,56 @@ class Engine:
         self.layers.append(L)
         return L
 
+    def stem_gn_ok(self, x: Tensor, f: int) -> bool:
+        """can the input block run fused (``stem_block``)?  bf16 storage, one image channel, 16 features, and a backend
+        with the fused kernels (the emulated CPU backend and the fp32 parity mode keep the per-branch calls)"""
+        ok = getattr(self.be, "stem_gn_ok", None)
+        return ok is not None and self.T == torch.bfloat16 and f == 16 and ok(x, f, self.dims)
+
+    def stem_block(self, x: Tensor, sp0, f: int, out: Tensor, drop: bool) -> Tuple[Layer, Layer]:
+        """InputTransition (VNet3d.py:34-43, ResNet3d.py:24-41): relu(bn1(conv1(x))) + relu(bn1(conv2(x))) with the
+        dropout of each branch, in two launches -- the statistics of both branches, then the normalised sum written
+        into ``out``.  The raw stem outputs are never stored: both passes recompute them from the image."""
+        n = x.shape[0]
+        La = Layer(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", x=x)
+        Lb = Layer(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", x=x)
+        self._tag(La.wname)
+        for L in (La, Lb):
+            L.wpk = self._packs.get((L.wname, "fwd"))
+            if L.wpk is None:
+                L.wpk = self.be.pack_weight(self.P[L.wname], L.kind, "fwd", self.T, self.dims,
+                                            vox=sp0[0] * sp0[1] * sp0[2])
+        stats = [self.zeros((n, f, 2), torch.float64, x.device) for _ in range(2)]
+        P = self.P
+        self.be.stem_gn_stats(x, La.wpk, P[La.bname], Lb.wpk, P[Lb.bname], stats[0], stats[1])
+        if self._deferred is not None:
+            self._launch_deferred()                    # behind the first launch of the pass
+        vox = sp0[0] * sp0[1] * sp0[2]
+        for L, st in zip((La, Lb), stats):             # the masks in branch order, as conv_gn draws them
+            L.scale = self._next_mask() if drop else None
+            L.gn = (st, P[L.gname + ".weight"], P[L.gname + ".bias"], L.scale, vox, GROUPS, GN_EPS)
+            self.layers.append(L)
+        self._tag(La.wname)
+        self.be.stem_gn_apply(x, La.wpk, P[La.bname], Lb.wpk, P[Lb.bname], La.gn, Lb.gn, out)
+        return La, Lb
+
+    def stem_block_backward(self, La: Layer, Lb: Layer, g: Tensor) -> None:
+        """Backward of ``stem_block`` (no data gradient): the GroupNorm-backward sums of both branches in one pass
+        over g, then dy of both branches formed on chip and consumed there by both stem weight gradients (+ d gamma,
+        d beta and both bias gradients) in a second one."""
+        be, P, dev = self.be, self.P, g.device
+        self._tag(La.wname)
+        n, f = g.shape[0], g.shape[-1]
+        sums = [self.zeros((n, f, 3), torch.float64, dev) for _ in range(2)]
+        be.stem_gn_bwd_sums(La.x, La.wpk, P[La.bname], Lb.wpk, P[Lb.bname], La.gn, Lb.gn, g, sums[0], sums[1])
+        dwa = self.zeros((_taps(La.kind, self.dims), 1, f), torch.float32, dev)
+        dwb = self.zeros((1, 1, f), torch.float32, dev)
+        gv = self._grad_view
+        be.stem_gn_bwd(La.x, La.wpk, P[La.bname], Lb.wpk, P[Lb.bname], La.gn, Lb.gn, g, sums[0], sums[1], dwa, dwb,
+                       gv(La.gname + ".weight"), gv(La.gname + ".bias"), gv(La.bname), gv(Lb.bname))
+        self._unpack_list.append((dwa, gv(La.wname)))
+        self._unpack_list.append((dwb, gv(Lb.wname)))
+
     def head(self, wname: str, bname: str, x: Tensor, sp0, ncls: int) -> Tuple[Layer, Tensor, Optional[Tensor]]:
         """OutputTransition3d / UNet head: 1x1 conv to the classes + sigmoid/softmax (VNet3d.py:90-99).
         Inference form (``mask_threshold`` set; predict, model/modelVNet.py:655-676): the uint8 mask directly."""
@@ -551,9 +602,13 @@ class Engine:
         self._prepack(specs, need_grad, n_early=5)         # in_tr (2) + down_tr32 (down conv + 2 ops)
 
         # ---- InputTransition3d (VNet3d.py:34-43): one bn1 serves both branches
-        La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f)
-        Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f)
-        out = self.act(La, skips[0], L2=Lb)
+        if self.stem_gn_ok(xin, f):
+            La, Lb = self.stem_block(xin, sp0, f, skips[0], drop=True)
+            out = skips[0]
+        else:
+            La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f)
+            Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f)
+            out = self.act(La, skips[0], L2=Lb)
         sv["in_tr"] = (La, Lb)
 
         # ---- DownTransition3d x4 (VNet3d.py:55-59)
@@ -633,8 +688,11 @@ class Engine:
                 self._flush_bucket("down_tr256.down_conv.weight")
                 self._early_unpack()
         La, Lb = sv["in_tr"]
-        self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
-        self.bwd_layer(Lb, g, False)
+        if La.wpk is not None:
+            self.stem_block_backward(La, Lb, g)
+        else:
+            self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
+            self.bwd_layer(Lb, g, False)
         self._finish_backward()
         return flat
 
@@ -676,9 +734,13 @@ class Engine:
         self._prepack(specs, need_grad, n_early=5)         # in_tr (2) + down_tr32 (down conv + 2 ops)
 
         # ---- InputTransition3d (ResNet3d.py:24-41): one bn1 for both branches, no dropout
-        La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f, drop=False)
-        Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f, drop=False)
-        out = self.act(La, self.new(x, sp0, f), L2=Lb)
+        if self.stem_gn_ok(xin, f):
+            out = self.new(x, sp0, f)
+            La, Lb = self.stem_block(xin, sp0, f, out, drop=False)
+        else:
+            La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f, drop=False)
+            Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f, drop=False)
+            out = self.act(La, self.new(x, sp0, f), L2=Lb)
         sv["in_tr"] = (La, Lb)
 
         # ---- DownTransition3d x4 (ResNet3d.py:44-58): the LUConv stacks have no dropout
@@ -736,8 +798,11 @@ class Engine:
                 self._flush_bucket("down_tr256.down_conv.weight")
                 self._early_unpack()
         La, Lb = sv["in_tr"]
-        self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
-        self.bwd_layer(Lb, g, False)
+        if La.wpk is not None:
+            self.stem_block_backward(La, Lb, g)
+        else:
+            self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
+            self.bwd_layer(Lb, g, False)
         self._finish_backward()
         return flat
 

@@ -1,6 +1,6 @@
 """Per-kernel timings at the VNet3d 96^3 / batch-2 layer shapes, through the C ABI (one GPU).
 
-    python tools/microbench_ops.py [--reps 20] [--only stem,gn,pack,wgrad,conv]
+    python tools/microbench_ops.py [--reps 20] [--only stem,stemgn,gn,pack,wgrad,conv]
 
 Every op is timed with CUDA events on the current stream, once with a warm L2 (back-to-back launches) and
 once "cold" (a 256 MiB write between launches, the way bench.py flushes between steps).  This is a
@@ -116,6 +116,36 @@ def bench_stem(be, tm, n, s):
                bytes_=vox * (4 + 32), flops=2 * vox * taps * 16)
 
 
+def bench_stem_gn(be, tm, n, s):
+    """the fused input block (csrc/stem_gn.cu): its four launches, beside the nine per-branch launches they replace
+    (algorithmic bytes: image 4 B/voxel, 16-channel bf16 tensors 32 B/voxel)"""
+    vox = n * s ** 3
+    x = rnd((n, s, s, s, 1), torch.float32)
+    p3 = be.pack_weight(rnd((16, 1, 3, 3, 3), torch.float32, 0.2), K3, "fwd", torch.bfloat16, 3, vox=s ** 3)
+    p1 = be.pack_weight(rnd((16, 1, 1, 1, 1), torch.float32, 0.2), K1, "fwd", torch.bfloat16, 3, vox=s ** 3)
+    b3, b1 = rnd((16,), torch.float32, 0.1), rnd((16,), torch.float32, 0.1)
+    gamma, beta = rnd((16,), torch.float32) + 1.0, rnd((16,), torch.float32, 0.1)
+    st = [torch.zeros((n, 16, 2), dtype=torch.float64, device=DEV) for _ in range(2)]
+    be.stem_gn_stats(x, p3, b3, p1, b1, st[0], st[1])
+    scale = torch.full((n, 16), 1.25, dtype=torch.float32, device=DEV)
+    gn3, gn1 = ((st[i], gamma, beta, scale, s ** 3, 8, 1e-5) for i in range(2))
+    cat = torch.empty((n, s, s, s, 32), dtype=torch.bfloat16, device=DEV)
+    g = rnd((n, s, s, s, 16))
+    sums = [torch.zeros((n, 16, 3), dtype=torch.float64, device=DEV) for _ in range(2)]
+    be.stem_gn_bwd_sums(x, p3, b3, p1, b1, gn3, gn1, g, sums[0], sums[1])
+    dw3, dw1 = torch.zeros((27, 1, 16), device=DEV), torch.zeros((1, 1, 16), device=DEV)
+    d16 = [torch.zeros(16, device=DEV) for _ in range(4)]
+    tm.run(f"stem_gn_stats       2x1->16 @{s}^3", lambda: be.stem_gn_stats(x, p3, b3, p1, b1, st[0], st[1]),
+           bytes_=vox * 4)
+    tm.run(f"stem_gn_apply       2x1->16 @{s}^3", lambda: be.stem_gn_apply(x, p3, b3, p1, b1, gn3, gn1, cat[..., 16:]),
+           bytes_=vox * (4 + 32))
+    tm.run(f"stem_gn_bwd_sums    2x1->16 @{s}^3",
+           lambda: be.stem_gn_bwd_sums(x, p3, b3, p1, b1, gn3, gn1, g, sums[0], sums[1]), bytes_=vox * (4 + 32))
+    tm.run(f"stem_gn_bwd         2x1->16 @{s}^3",
+           lambda: be.stem_gn_bwd(x, p3, b3, p1, b1, gn3, gn1, g, sums[0], sums[1], dw3, dw1, *d16),
+           bytes_=vox * (4 + 32))
+
+
 def bench_gn(be, tm, n):
     for c, s in ((16, 96), (32, 96), (32, 48), (64, 24), (128, 12), (256, 6)):
         vox = s ** 3
@@ -214,7 +244,7 @@ def bench_convbwd(be, tm, n):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=7)
-    ap.add_argument("--only", default="stem,gn,pack,wgrad,conv")
+    ap.add_argument("--only", default="stem,stemgn,gn,pack,wgrad,conv")
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--tag", default="run")
     ap.add_argument("--eager", action="store_true", help="launch every op twice without graphs/timing (ncu runs)")
@@ -225,6 +255,8 @@ def main():
     with torch.no_grad():
         if "stem" in which:
             bench_stem(be, tm, a.batch, 96)
+        if "stemgn" in which:
+            bench_stem_gn(be, tm, a.batch, 96)
         if "gn" in which:
             bench_gn(be, tm, a.batch)
         if "pack" in which:
