@@ -43,6 +43,12 @@ extern "C" {
 #define B200SEG_I64 16 /* labels only: int64 class indices (model/dataset.py:114); B200SEG_F32 = soft binary targets */
 #define B200SEG_U8 17  /* masks only: one byte per voxel (bool or uint8) */
 #define B200SEG_I32 18 /* masks only: int32 */
+#define B200SEG_I16 19 /* resampled volumes only: int16 */
+
+/* intensity steps of b200seg_resample_linear / b200seg_normalize */
+#define B200SEG_NORM_NONE 0    /* resample only */
+#define B200SEG_NORM_MEANSTD 1 /* truncate to [lower, upper], then (x - mean) / sigma (N - 1) */
+#define B200SEG_NORM_PCTL 2    /* dataprocess/utils.py normalize(): 5/95 percentile clip, z-score of the nonzero voxels */
 
 /* conv kinds */
 #define B200SEG_K3 0    /* 3x3x3 (dims==3) or 1x3x3 (dims==2), stride 1, zero pad 1 */
@@ -439,6 +445,32 @@ int b200seg_stage_u8_normalize(const uint8_t* img, int n, int64_t per_sample, co
                                int out_dtype, int device, b200seg_stream stream);
 int b200seg_stage_labels_u8(const uint8_t* lab, int64_t count, int binarize, int64_t* out, int device,
                             b200seg_stream stream);
+
+/* ---- whole-volume 3-D inference (XModel.inference / inference_patch, model/modelVNet.py:678-698,
+ * model/modelUnet.py:684-763): SimpleITK's resamples and the intensity normalisations around the network.  Volumes
+ * are dense [D][H][W]; ratio_zyx (host fp64 [3], read during the call) is the input-index step per output index
+ * along D, H, W (S_in / S_out, or new spacing / old spacing).  A sample exists where -0.5 <= i * r < S_in - 0.5 on
+ * every axis (ITK's inside-buffer rule), else the output is 0.
+ * b200seg_resample_linear: trilinear sample in fp64 (lerps along W, H, then D), cast to the input's pixel type
+ * (src_dtype B200SEG_U8, B200SEG_I16, B200SEG_I32: clamped to the type's range, truncated toward zero; B200SEG_F32:
+ * rounded), then written as fp32 to out [oD][oH][oW].  norm_mode B200SEG_NORM_MEANSTD also truncates to [lower,
+ * upper] and writes per-block fp64 sums to the workspace; B200SEG_NORM_PCTL writes the sort keys there
+ * (B200SEG_NORM_NONE needs no workspace).
+ * b200seg_normalize: x (the resample's output, same norm_mode and workspace) -> out, a separate buffer.  The workspace's
+ * first 64 bytes hold fp64 stats {mean, sigma, p5, p95, unchanged flag, count}: MEANSTD uses the N - 1 deviation of
+ * all voxels; PCTL the numpy 'linear' 5th / 95th percentiles, then the mean and population deviation of the nonzero
+ * clipped voxels, and the flag is 1 where normalize() returns the clipped volume unchanged (a std of 0).
+ * b200seg_resample_nearest_u8: out [oD][oH][oW] uint8; voxels with an index >= (vD, vH, vW) on any axis are 0,
+ * the rest take src at floor(i * r + 0.5).
+ * Sizes >= 1; the PCTL network grid holds < 2^31 voxels.  Every reduction has a fixed order. */
+int64_t b200seg_resample_workspace(int norm_mode, int oD, int oH, int oW);
+int b200seg_resample_linear(const void* src, int src_dtype, int D, int H, int W, const double* ratio_zyx, int oD,
+                            int oH, int oW, int norm_mode, float lower, float upper, float* out, void* workspace,
+                            int64_t workspace_bytes, int device, b200seg_stream stream);
+int b200seg_normalize(int norm_mode, const float* x, int oD, int oH, int oW, void* workspace, int64_t workspace_bytes,
+                      float* out, int device, b200seg_stream stream);
+int b200seg_resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* ratio_zyx, int vD, int vH,
+                                int vW, int oD, int oH, int oW, uint8_t* out, int device, b200seg_stream stream);
 
 #ifdef __cplusplus
 }

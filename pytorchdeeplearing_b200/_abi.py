@@ -17,6 +17,8 @@ K3, K1, DOWN, UP = 0, 1, 2, 3
 F32, BF16, BF16_TC, BF16_HALO, BF16_HALO_WS = 0, 1, 2, 3, 4
 I64 = 16
 U8, I32 = 17, 18          # mask dtypes of the segmentation metrics
+I16 = 19                  # volumes of the whole-volume resample
+NORM_NONE, NORM_MEANSTD, NORM_PCTL = 0, 1, 2
 # kernel families of b200seg_conv / b200seg_wgrad (include/b200seg.h: B200SEG_CONV_*, B200SEG_WGRAD_*)
 CONV_PATHS = ("PW_MMA", "TC", "HALO2D", "HALO3", "HALO_WS", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
 WGRAD_PATHS = ("HALO_MMA", "TC", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
@@ -120,6 +122,10 @@ _SIGNATURES = {
     "b200seg_stage_u8_sums": ([_vp, _i, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_stage_u8_normalize": ([_vp, _i, _i64, _vp, _vp, _i, _i, _vp], C.c_int),
     "b200seg_stage_labels_u8": ([_vp, _i64, _i, _vp, _i, _vp], C.c_int),
+    "b200seg_resample_workspace": ([_i, _i, _i, _i], C.c_int64),
+    "b200seg_resample_linear": ([_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _vp, _vp, _i64, _i, _vp], C.c_int),
+    "b200seg_normalize": ([_i, _vp, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
+    "b200seg_resample_nearest_u8": ([_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -847,6 +853,43 @@ class CudaBackend:
         self._check(self.lib.b200seg_stage_labels_u8(lab.data_ptr(), lab.numel(), 1 if binarize else 0, out.data_ptr(),
                                                      dev, st))
         return out
+
+    # ------------------------------------------------------------------ whole-volume 3-D inference (csrc/resample.cu)
+    _VOL_DTYPES = {torch.uint8: U8, torch.int16: I16, torch.int32: I32, torch.float32: F32}
+
+    def resample_workspace(self, mode, out_zyx, device):
+        """uint8 workspace of b200seg_resample_workspace bytes; its first 8 fp64 are the stats of b200seg_normalize"""
+        nb = int(self.lib.b200seg_resample_workspace(mode, *out_zyx))
+        return torch.empty(max(nb, 256), dtype=torch.uint8, device=device)
+
+    def resample_linear(self, src, ratio_zyx, out, mode=NORM_NONE, lower=0.0, upper=0.0, ws=None):
+        """src dense (D, H, W) uint8 / int16 / int32 / fp32 -> out dense fp32 (oD, oH, oW); ratio_zyx host floats"""
+        dev, st = self._ds(src)
+        code = self._VOL_DTYPES.get(src.dtype)
+        if code is None:
+            raise TypeError(f"volumes must be uint8, int16, int32 or float32, got {src.dtype}")
+        assert src.dim() == 3 and src.is_contiguous() and out.dim() == 3 and out.is_contiguous()
+        assert out.dtype == torch.float32
+        r = (C.c_double * 3)(*[float(v) for v in ratio_zyx])
+        self._check(self.lib.b200seg_resample_linear(src.data_ptr(), code, *src.shape, C.cast(r, _vp), *out.shape, mode,
+                                                     lower, upper, out.data_ptr(), _p(ws),
+                                                     0 if ws is None else ws.numel(), dev, st))
+
+    def normalize(self, mode, x, ws, out):
+        """x: the fp32 output of resample_linear(..., mode, ws=ws) -> out (a separate fp32 buffer of x's size)"""
+        dev, st = self._ds(x)
+        assert x.dim() == 3 and x.is_contiguous() and out.is_contiguous() and out.numel() == x.numel()
+        self._check(self.lib.b200seg_normalize(mode, x.data_ptr(), *x.shape, ws.data_ptr(), ws.numel(), out.data_ptr(),
+                                               dev, st))
+
+    def resample_nearest_u8(self, src, ratio_zyx, valid_zyx, out):
+        """src dense uint8 (D, H, W) -> out dense uint8: the NN resample in the valid corner, 0 elsewhere"""
+        dev, st = self._ds(src)
+        assert src.dtype == torch.uint8 and out.dtype == torch.uint8 and src.dim() == 3 and out.dim() == 3
+        assert src.is_contiguous() and out.is_contiguous()
+        r = (C.c_double * 3)(*[float(v) for v in ratio_zyx])
+        self._check(self.lib.b200seg_resample_nearest_u8(src.data_ptr(), *src.shape, C.cast(r, _vp), *valid_zyx,
+                                                         *out.shape, out.data_ptr(), dev, st))
 
     def mask_logits(self, logits, threshold, mask):
         dev, st = self._ds(logits)

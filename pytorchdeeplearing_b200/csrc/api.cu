@@ -162,6 +162,14 @@ int cls_head_bwd(const float* dlogits, const float* pooled, const float* hidden,
                  int Hd, int K, float* work, const b200seg_tensor* dx, float* dw1, float* db1, float* dw2, float* db2,
                  int device, cudaStream_t st);
 
+int64_t resample_workspace(int mode, long long nvox);
+int resample_linear(const void* src, int dtype, int D, int H, int W, const double* ratio, int oD, int oH, int oW,
+                    int mode, float lower, float upper, float* out, void* ws, long long ws_bytes, cudaStream_t st);
+int normalize_volume(int mode, const float* x, long long nvox, void* ws, long long ws_bytes, float* out, int device,
+                     cudaStream_t st);
+int resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* ratio, int vD, int vH, int vW, int oD,
+                        int oH, int oW, uint8_t* out, int device, cudaStream_t st);
+
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
          (t->dtype == B200SEG_F32 || t->dtype == B200SEG_BF16);
@@ -797,6 +805,56 @@ int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const
   B200_DEVICE(device);
   return ssim_bwd(dims, img1, strides1, img2, strides2, N, C, D, H, W, window_size, taps, coef, size_average, gout,
                   acc, grad1, grad2, device, ST(stream));
+}
+
+static bool valid_ratio(const double* r) {
+  return r && r[0] > 0.0 && r[1] > 0.0 && r[2] > 0.0 && r[0] < 1e9 && r[1] < 1e9 && r[2] < 1e9;
+}
+
+int64_t b200seg_resample_workspace(int norm_mode, int oD, int oH, int oW) {
+  if (norm_mode < B200SEG_NORM_NONE || norm_mode > B200SEG_NORM_PCTL || oD < 1 || oH < 1 || oW < 1) return 0;
+  return resample_workspace(norm_mode, (long long)oD * oH * oW);
+}
+
+int b200seg_resample_linear(const void* src, int src_dtype, int D, int H, int W, const double* ratio_zyx, int oD,
+                            int oH, int oW, int norm_mode, float lower, float upper, float* out, void* workspace,
+                            int64_t workspace_bytes, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(src && out, "b200seg_resample_linear: null argument");
+  B200_CHECK_ARG(D >= 1 && H >= 1 && W >= 1 && oD >= 1 && oH >= 1 && oW >= 1,
+                 "b200seg_resample_linear: sizes must be >= 1 (%d %d %d -> %d %d %d)", D, H, W, oD, oH, oW);
+  B200_CHECK_ARG(src_dtype == B200SEG_U8 || src_dtype == B200SEG_I16 || src_dtype == B200SEG_I32 ||
+                     src_dtype == B200SEG_F32,
+                 "b200seg_resample_linear: unsupported pixel type %d", src_dtype);
+  B200_CHECK_ARG(norm_mode >= B200SEG_NORM_NONE && norm_mode <= B200SEG_NORM_PCTL,
+                 "b200seg_resample_linear: bad norm_mode %d", norm_mode);
+  B200_CHECK_ARG(valid_ratio(ratio_zyx), "b200seg_resample_linear: ratios must be finite and > 0");
+  B200_CHECK_ARG(norm_mode != B200SEG_NORM_PCTL || (long long)oD * oH * oW < (1LL << 31),
+                 "b200seg_resample_linear: the percentile sort takes < 2^31 voxels");
+  B200_DEVICE(device);
+  return resample_linear(src, src_dtype, D, H, W, ratio_zyx, oD, oH, oW, norm_mode, lower, upper, out, workspace,
+                         workspace_bytes, ST(stream));
+}
+
+int b200seg_normalize(int norm_mode, const float* x, int oD, int oH, int oW, void* workspace, int64_t workspace_bytes,
+                      float* out, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(x && out && x != out, "b200seg_normalize: null or aliased argument");
+  B200_CHECK_ARG(oD >= 1 && oH >= 1 && oW >= 1, "b200seg_normalize: sizes must be >= 1");
+  B200_CHECK_ARG(norm_mode == B200SEG_NORM_MEANSTD || norm_mode == B200SEG_NORM_PCTL,
+                 "b200seg_normalize: bad norm_mode %d", norm_mode);
+  B200_CHECK_ARG(norm_mode != B200SEG_NORM_PCTL || (long long)oD * oH * oW < (1LL << 31),
+                 "b200seg_normalize: the percentile sort takes < 2^31 voxels");
+  B200_DEVICE(device);
+  return normalize_volume(norm_mode, x, (long long)oD * oH * oW, workspace, workspace_bytes, out, device, ST(stream));
+}
+
+int b200seg_resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* ratio_zyx, int vD, int vH,
+                                int vW, int oD, int oH, int oW, uint8_t* out, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(src && out, "b200seg_resample_nearest_u8: null argument");
+  B200_CHECK_ARG(D >= 1 && H >= 1 && W >= 1 && oD >= 1 && oH >= 1 && oW >= 1 && vD >= 0 && vH >= 0 && vW >= 0,
+                 "b200seg_resample_nearest_u8: bad sizes");
+  B200_CHECK_ARG(valid_ratio(ratio_zyx), "b200seg_resample_nearest_u8: ratios must be finite and > 0");
+  B200_DEVICE(device);
+  return resample_nearest_u8(src, D, H, W, ratio_zyx, vD, vH, vW, oD, oH, oW, out, device, ST(stream));
 }
 
 }  // extern "C"
