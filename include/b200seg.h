@@ -259,6 +259,29 @@ int b200seg_stem_gn_bwd(const b200seg_tensor* x, const void* w3, const float* b3
                         const double* sums1, float* dw3, float* dw1, float* dgamma, float* dbeta, float* db3,
                         float* db1, int device, b200seg_stream stream);
 
+/* ---- fused first layer of VNet3d's up_tr32 (VNet3d.py:62-72): up_conv, a 2x2x2 stride-2 transposed convolution of a
+ * bf16 32-channel input x to 16 channels at twice the resolution, then GroupNorm(8, 16), dropout and ReLU.  No pass
+ * stores the raw output y: each recomputes it from x with the arithmetic of b200seg_conv's pointwise mma.sync kernel,
+ * so the results equal b200seg_conv (stats) -> b200seg_apply_gn on the forward side and b200seg_gn_bwd_reduce_gn ->
+ * b200seg_gn_bwd_apply_gn -> b200seg_wgrad + the data-gradient b200seg_conv on the backward side.  w: the bf16 forward
+ * operand (b200seg_pack_weight, [8][16][32]); gn: the layer's GroupNorm reference (8 groups, vox = the fine grid's
+ * D*H*W); stats [N][16][2], sums [N][16][3] fp64, zero on entry where written.  Ask b200seg_up_gn_supported first. */
+int b200seg_up_gn_supported(const b200seg_tensor* x, int cout, int dims);
+/* per-(n, c) sum y, sum y^2 (what b200seg_conv writes into its stats argument) */
+int b200seg_up_gn_stats(const b200seg_tensor* x, const void* w, const float* bias, double* stats, int device,
+                        b200seg_stream stream);
+/* out = relu(y*A+B); out: bf16, 16 channels, the fine grid, 16-byte aligned rows (pitch a multiple of 8) */
+int b200seg_up_gn_apply(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                        const b200seg_tensor* out, int device, b200seg_stream stream);
+/* sums [N][16][3] += {sum g*m, sum g*m*y, sum y} (b200seg_gn_bwd_reduce_gn's layout) */
+int b200seg_up_gn_bwd_sums(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                           const b200seg_tensor* g, double* sums, int device, b200seg_stream stream);
+/* dw [8][16][32] += (b200seg_wgrad's layout for this layer), dx = the data gradient (bf16, 32 channels, the coarse
+ * grid), dgamma, dbeta [16] +=, dbias [16] += (may be NULL); dy itself never leaves the chip */
+int b200seg_up_gn_bwd(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                      const b200seg_tensor* g, const double* sums, float* dw, const b200seg_tensor* dx, float* dgamma,
+                      float* dbeta, float* dbias, int device, b200seg_stream stream);
+
 /* ---- nn.MaxPool3d/2d(2,2) (Unet3d.py:18-24) */
 int b200seg_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dims, int device, b200seg_stream stream);
 int b200seg_pool_bwd(const b200seg_tensor* x, const b200seg_tensor* g_out, const b200seg_tensor* addend,

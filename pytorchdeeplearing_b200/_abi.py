@@ -90,6 +90,11 @@ _SIGNATURES = {
     "b200seg_stem_gn_bwd_sums": ([_PT, _vp, _vp, _vp, _vp, _PG, _PG, _PT, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_stem_gn_bwd": ([_PT, _vp, _vp, _vp, _vp, _PG, _PG, _PT, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp],
                             C.c_int),
+    "b200seg_up_gn_supported": ([_PT, _i, _i], C.c_int),
+    "b200seg_up_gn_stats": ([_PT, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_up_gn_apply": ([_PT, _vp, _vp, _PG, _PT, _i, _vp], C.c_int),
+    "b200seg_up_gn_bwd_sums": ([_PT, _vp, _vp, _PG, _PT, _vp, _i, _vp], C.c_int),
+    "b200seg_up_gn_bwd": ([_PT, _vp, _vp, _PG, _PT, _vp, _vp, _PT, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_head_bwd_supported": ([_i, _i], C.c_int),
     "b200seg_head_bwd": ([_PT, _vp, _vp, _PT, _vp, _vp, _i, _i, _vp], C.c_int),
     "b200seg_loss_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _f, _vp, _vp, _i, _vp], C.c_int),
@@ -536,6 +541,39 @@ class CudaBackend:
                                                  C.byref(dg), sums3.data_ptr(), sums1.data_ptr(), dw3.data_ptr(),
                                                  dw1.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), _p(db3),
                                                  _p(db1), dev, st))
+
+    # ------------------------------------------------------------------ fused first layer of up_tr32 (csrc/up_gn.cu)
+    # w: the packed forward operand of the transposed convolution (pack_weight(..., "fwd", torch.bfloat16, ...) on the
+    # pointwise mma.sync path); the raw output is never stored: every call recomputes it from x (N,D,H,W,32)
+    def up_gn_ok(self, x, wpk, cout, dims):
+        """can the fused up_tr32 kernels take this input (3-D, bf16, 32 -> 16 channels) and forward operand?"""
+        if x.dtype != torch.bfloat16 or x.dim() != 5 or wpk is None or wpk.code != BF16_TC:
+            return False
+        return bool(self.lib.b200seg_up_gn_supported(C.byref(_desc(x)), cout, dims))
+
+    def up_gn_stats(self, x, wpk, bias, stats):
+        dev, st = self._ds(x)
+        self._check(self.lib.b200seg_up_gn_stats(C.byref(_desc(x)), wpk.t.data_ptr(), _p(bias), stats.data_ptr(),
+                                                 dev, st))
+
+    def up_gn_apply(self, x, wpk, bias, gn, out):
+        dev, st = self._ds(x)
+        gg, do = self._gn(gn), _desc(out)
+        self._check(self.lib.b200seg_up_gn_apply(C.byref(_desc(x)), wpk.t.data_ptr(), _p(bias), C.byref(gg),
+                                                 C.byref(do), dev, st))
+
+    def up_gn_bwd_sums(self, x, wpk, bias, gn, g, sums):
+        dev, st = self._ds(x)
+        gg, dg = self._gn(gn), _desc(g)
+        self._check(self.lib.b200seg_up_gn_bwd_sums(C.byref(_desc(x)), wpk.t.data_ptr(), _p(bias), C.byref(gg),
+                                                    C.byref(dg), sums.data_ptr(), dev, st))
+
+    def up_gn_bwd(self, x, wpk, bias, gn, g, sums, dw, dx, dgamma, dbeta, dbias):
+        dev, st = self._ds(x)
+        gg, dg, dd = self._gn(gn), _desc(g), _desc(dx)
+        self._check(self.lib.b200seg_up_gn_bwd(C.byref(_desc(x)), wpk.t.data_ptr(), _p(bias), C.byref(gg), C.byref(dg),
+                                               sums.data_ptr(), dw.data_ptr(), C.byref(dd), dgamma.data_ptr(),
+                                               dbeta.data_ptr(), _p(dbias), dev, st))
 
     def gn_bwd_reduce(self, g, y, coef, sums):
         dev, st = self._ds(y)

@@ -58,6 +58,10 @@ int stem_gn(int mode, const b200seg_tensor* x, const void* wa, const float* ba, 
             const b200seg_gn* gna, const b200seg_gn* gnb, double* stats_a, double* stats_b,
             const b200seg_tensor* out, const b200seg_tensor* gr, double* sums_a, double* sums_b, float* dwa,
             float* dwb, float* dgamma, float* dbeta, float* dba, float* dbb, int device, cudaStream_t st);
+int up_gn_supported(const b200seg_tensor* x, int cout, int dims);
+int up_gn(int mode, const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn, double* stats,
+          const b200seg_tensor* out, const b200seg_tensor* gr, double* sums, float* dw, const b200seg_tensor* dx,
+          float* dgamma, float* dbeta, float* dbias, int device, cudaStream_t st);
 int stem_conv_supported(int kind, const b200seg_tensor* x, const b200seg_tensor* y, const b200seg_tensor* addend);
 int stem_conv(int kind, int dims, const b200seg_tensor* x, const void* w, int w_dtype, const float* bias,
               const b200seg_tensor* y, double* stats, int device, cudaStream_t st);
@@ -524,6 +528,48 @@ int b200seg_stem_gn_bwd(const b200seg_tensor* x, const void* w3, const float* b3
   B200_DEVICE(device);
   return stem_gn(3, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, nullptr, g, const_cast<double*>(sums3),
                  const_cast<double*>(sums1), dw3, dw1, dgamma, dbeta, db3, db1, device, ST(stream));
+}
+
+int b200seg_up_gn_supported(const b200seg_tensor* x, int cout, int dims) {
+  if (x == nullptr || !valid_tensor(x)) return 0;
+  return up_gn_supported(x, cout, dims);
+}
+
+int b200seg_up_gn_stats(const b200seg_tensor* x, const void* w, const float* bias, double* stats, int device,
+                        b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  B200_DEVICE(device);
+  return up_gn(0, x, w, bias, nullptr, stats, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+               device, ST(stream));
+}
+
+int b200seg_up_gn_apply(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                        const b200seg_tensor* out, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(out, "out");
+  B200_DEVICE(device);
+  return up_gn(1, x, w, bias, gn, nullptr, out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, device,
+               ST(stream));
+}
+
+int b200seg_up_gn_bwd_sums(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                           const b200seg_tensor* g, double* sums, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(g, "g");
+  B200_DEVICE(device);
+  return up_gn(2, x, w, bias, gn, nullptr, nullptr, g, sums, nullptr, nullptr, nullptr, nullptr, nullptr, device,
+               ST(stream));
+}
+
+int b200seg_up_gn_bwd(const b200seg_tensor* x, const void* w, const float* bias, const b200seg_gn* gn,
+                      const b200seg_tensor* g, const double* sums, float* dw, const b200seg_tensor* dx, float* dgamma,
+                      float* dbeta, float* dbias, int device, b200seg_stream stream) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(g, "g");
+  REQ_TENSOR(dx, "dx");
+  B200_DEVICE(device);
+  return up_gn(3, x, w, bias, gn, nullptr, nullptr, g, const_cast<double*>(sums), dw, dx, dgamma, dbeta, dbias, device,
+               ST(stream));
 }
 
 int b200seg_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dims, int device, b200seg_stream stream) {

@@ -11,19 +11,9 @@
 //     (m16n8k16, fp32 accumulators);
 //   * epilogue on the accumulator fragments: + bias, GroupNorm statistics (per-lane column partials, folded once per
 //     sample), + addend, bf16x2 stores.
-#include "common.cuh"
+#include "pw_mma.cuh"
 
 namespace b200seg {
-
-constexpr int PW_TILE = 512;            // voxels per CTA step
-constexpr int PW_THREADS = 256;
-
-__device__ __forceinline__ void pw_mma(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // UP = false: 1x1x1 conv.  UP = true: k2s2 transposed conv (VNet3d.py:62 up_conv and the data gradient of the k2s2
 // down conv): the same A fragments are multiplied by the 8 (4 in 2-D) tap matrices and every product row is stored
@@ -43,7 +33,7 @@ __global__ void __launch_bounds__(PW_THREADS, UP ? 1 : 2)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gq = lane >> 2, tq = lane & 3;
 
-  // weights -> B fragments: b0 = (k = 2t, 2t+1 ; n = g), b1 = (k = 2t+8, 2t+9 ; n = g); w is [tap][n][k], k contiguous
+  // weights -> B fragments (held in registers for the kernel's lifetime)
   constexpr int TAPS = UP ? 8 : 1;
   const int taps = UP ? 4 * ud : 1;                 // 2-D transposed conv: 4 taps
   uint32_t wb[TAPS][KS][NT][2];
@@ -52,11 +42,8 @@ __global__ void __launch_bounds__(PW_THREADS, UP ? 1 : 2)
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
-      for (int nt = 0; nt < NT; ++nt) {
-        const bf16* wr = w + ((tp < taps ? tp : 0) * COUT + nt * 8 + gq) * CIN + ks * 16 + 2 * tq;
-        wb[tp][ks][nt][0] = *reinterpret_cast<const uint32_t*>(wr);
-        wb[tp][ks][nt][1] = *reinterpret_cast<const uint32_t*>(wr + 8);
-      }
+      for (int nt = 0; nt < NT; ++nt)
+        pw_b_frag<CIN, COUT>(w, tp < taps ? tp : 0, ks, nt, gq, tq, wb[tp][ks][nt][0], wb[tp][ks][nt][1]);
   float bv[NT][2];
 #pragma unroll
   for (int nt = 0; nt < NT; ++nt) {
@@ -115,8 +102,7 @@ __global__ void __launch_bounds__(PW_THREADS, UP ? 1 : 2)
   load_tile(0, first);
   asm volatile("cp.async.wait_all;" ::: "memory");
   __syncthreads();
-  // ldmatrix (non-transposed) lane address: matrix m = lane >> 3 -> (voxel half m & 1, channel half m >> 1)
-  const int a_lane = (((lane >> 3) & 1) * 8 + (lane & 7)) * XP + (lane >> 4) * 16;
+  const int a_lane = pw_a_lane(lane, XP);
   long long cur_n = first * PW_TILE / V;
   for (long long tile = first; tile < last; ++tile) {
     const int buf = (int)((tile - first) & 1);
@@ -131,35 +117,16 @@ __global__ void __launch_bounds__(PW_THREADS, UP ? 1 : 2)
     for (int mi = 0; mi < PW_TILE / (8 * 16); ++mi) {
       const int r0 = (warp * (PW_TILE / 8) + mi * 16);          // first voxel row of this 16-row group in the tile
       uint32_t a[KS][4];
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks)
-        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                     : "=r"(a[ks][0]), "=r"(a[ks][1]), "=r"(a[ks][2]), "=r"(a[ks][3])
-                     : "r"(xs + (uint32_t)(r0 * XP + a_lane + ks * 32)));
+      pw_a_frags<KS>(a, xs, r0 * XP + a_lane);
       const long long v0 = tile * PW_TILE + r0;        // first (coarse) voxel of the group
       long long ob = v0;                               // UP: fine voxel of coarse voxel v0 at tap (0,0,0)
       int fw = 0, fh = 0;
-      if (UP) {
-        const long long vs = v0 % V;
-        const long long ns = v0 / V;
-        const int cw = (int)(vs % W), ch = (int)((vs / W) % H), cd = (int)(vs / ((long long)W * H));
-        fw = 2 * W;
-        fh = 2 * H;
-        ob = ((ns * (D * ud) + (long long)cd * ud) * fh + 2 * ch) * fw + 2 * cw;
-      }
+      if (UP) ob = pw_up_base(v0, V, D, H, W, ud, fw, fh);
 #pragma unroll
       for (int tp = 0; tp < TAPS; ++tp) {
         if (UP && tp >= taps) break;
         float acc[NT][4];
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          acc[nt][0] = acc[nt][2] = bv[nt][0];
-          acc[nt][1] = acc[nt][3] = bv[nt][1];
-        }
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-          for (int nt = 0; nt < NT; ++nt) pw_mma(acc[nt], a[ks], wb[tp][ks][nt][0], wb[tp][ks][nt][1]);
+        pw_chain<KS, NT>(acc, a, wb[tp], bv);
         if (stats != nullptr) {
 #pragma unroll
           for (int nt = 0; nt < NT; ++nt) {

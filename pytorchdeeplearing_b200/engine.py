@@ -407,6 +407,54 @@ class Engine:
         self._unpack_list.append((dwa, gv(La.wname)))
         self._unpack_list.append((dwb, gv(Lb.wname)))
 
+    def up_gn_ok(self, x: Tensor, wname: str, co: int) -> bool:
+        """can this transposed-conv layer run fused (``up_block``)?  bf16 storage, 3-D, 32 -> 16 channels at the shapes of
+        the pointwise mma.sync kernel, and a backend with the fused kernels (the emulated CPU backend and the fp32
+        parity mode keep the per-layer calls)"""
+        ok = getattr(self.be, "up_gn_ok", None)
+        if ok is None or self.T != torch.bfloat16 or self.dims != 3:
+            return False
+        return ok(x, self._packs.get((wname, "fwd")), co, self.dims)
+
+    def up_block(self, name: str, x: Tensor, sp, co: int, out: Tensor) -> Layer:
+        """UpTransition's up_conv -> bn -> Dropout -> ReLU (VNet3d.py:62-72) in two launches -- the statistics, then the
+        normalised activation written into ``out`` (the left half of the skip concat).  The raw transposed-conv output
+        is never stored: both passes recompute it from ``x``."""
+        L = Layer(UP, name + ".up_conv.weight", name + ".up_conv.bias", name + ".bn", x=x)
+        self._tag(L.wname)
+        if L.wname in self._late:
+            if self._deferred is not None:
+                self._launch_deferred()
+            self._join_fwd_side()
+        L.wpk = self._packs[(L.wname, "fwd")]
+        n = x.shape[0]
+        stats = self.zeros((n, co, 2), torch.float64, x.device)
+        P = self.P
+        self.be.up_gn_stats(x, L.wpk, P[L.bname], stats)
+        L.scale = self._next_mask()
+        L.gn = (stats, P[L.gname + ".weight"], P[L.gname + ".bias"], L.scale, sp[0] * sp[1] * sp[2], GROUPS, GN_EPS)
+        self.layers.append(L)
+        self.be.up_gn_apply(x, L.wpk, P[L.bname], L.gn, out)
+        return L
+
+    def up_block_backward(self, L: Layer, g: Tensor) -> Tensor:
+        """Backward of ``up_block``: the GroupNorm-backward sums in one pass over g, then dy formed on chip and consumed
+        there by the weight gradient and the data gradient (+ d gamma, d beta and the bias gradient) in a second one.
+        Returns the gradient w.r.t. the layer input."""
+        be, dev = self.be, g.device
+        self._tag(L.wname)
+        n, co = g.shape[0], g.shape[-1]
+        sums = self.zeros((n, co, 3), torch.float64, dev)
+        bias = self.P[L.bname]
+        be.up_gn_bwd_sums(L.x, L.wpk, bias, L.gn, g, sums)
+        dwp = self.zeros((_taps(UP, self.dims), co, L.x.shape[-1]), torch.float32, dev)
+        dx = torch.empty(L.x.shape, dtype=self.T, device=dev)
+        gv = self._grad_view
+        be.up_gn_bwd(L.x, L.wpk, bias, L.gn, g, sums, dwp, dx, gv(L.gname + ".weight"), gv(L.gname + ".bias"),
+                     gv(L.bname))
+        self._unpack_list.append((dwp, gv(L.wname)))
+        return dx
+
     def head(self, wname: str, bname: str, x: Tensor, sp0, ncls: int) -> Tuple[Layer, Tensor, Optional[Tensor]]:
         """OutputTransition3d / UNet head: 1x1 conv to the classes + sigmoid/softmax (VNet3d.py:90-99).
         Inference form (``mask_threshold`` set; predict, model/modelVNet.py:655-676): the uint8 mask directly."""
@@ -635,8 +683,11 @@ class Engine:
         nconvs = {"up_tr256": 3, "up_tr128": 3, "up_tr64": 2, "up_tr32": 1}
         for i, name in zip((3, 2, 1, 0), ["up_tr256", "up_tr128", "up_tr64", "up_tr32"]):
             co, sp = ch[i], sps[i]
-            Lu = self.conv_gn(UP, name + ".up_conv.weight", name + ".up_conv.bias", name + ".bn", out, sp, co)
-            self.act(Lu, cats[i][..., :co])                              # left half of the concat
+            if name == "up_tr32" and self.up_gn_ok(out, name + ".up_conv.weight", co):
+                Lu = self.up_block(name, out, sp, co, cats[i][..., :co])
+            else:
+                Lu = self.conv_gn(UP, name + ".up_conv.weight", name + ".up_conv.bias", name + ".bn", out, sp, co)
+                self.act(Lu, cats[i][..., :co])                          # left half of the concat
             Lc = self.conv_gn(K1, name + ".conv.weight", name + ".conv.bias", name + ".bn", cats[i], sp, co)
             xcat = self.act(Lc, self.new(x, sp, co))
             h, ops = xcat, []
@@ -673,9 +724,12 @@ class Engine:
                 gh = self.bwd_layer(ops[j], gh, True, dx_addend=g_out if j == 0 else None,
                                     prev=ops[j - 1] if j > 0 else Lc)
             gcat = self.bwd_layer(Lc, gh, True)          # (N,..,2*co)
-            co = Lu.y.shape[-1]
+            co = Lc.y.shape[-1]
             gskip[i] = gcat[..., co:]
-            g = self.bwd_layer(Lu, gcat[..., :co], True)
+            if Lu.wpk is not None:
+                g = self.up_block_backward(Lu, gcat[..., :co])
+            else:
+                g = self.bwd_layer(Lu, gcat[..., :co], True)
         for i, name in zip((3, 2, 1, 0), ["down_tr256", "down_tr128", "down_tr64", "down_tr32"]):
             Ld, ops = sv[name]
             g_out = g

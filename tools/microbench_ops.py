@@ -1,6 +1,6 @@
 """Per-kernel timings at the VNet3d 96^3 / batch-2 layer shapes, through the C ABI (one GPU).
 
-    python tools/microbench_ops.py [--reps 20] [--only stem,stemgn,gn,pack,wgrad,conv]
+    python tools/microbench_ops.py [--reps 20] [--only stem,stemgn,up,gn,pack,wgrad,conv]
 
 Every op is timed with CUDA events on the current stream, once with a warm L2 (back-to-back launches) and
 once "cold" (a 256 MiB write between launches, the way bench.py flushes between steps).  This is a
@@ -146,6 +146,56 @@ def bench_stem_gn(be, tm, n, s):
            bytes_=vox * (4 + 32))
 
 
+def bench_up(be, tm, n, s=96):
+    """the first layer of up_tr32 (UP 32@48^3 -> 16@96^3, GroupNorm, Dropout, ReLU into the concat's left half): the
+    six per-layer launches of forward and backward, and the GroupNorm-backward reduce of up_tr32.ops.0
+    (algorithmic bytes: X = the 32-channel coarse input, T = one 16-channel fine tensor)"""
+    c, ci, sc = 16, 32, s // 2
+    X, T = n * sc ** 3 * ci * 2, n * s ** 3 * c * 2
+    x = rnd((n, sc, sc, sc, ci))
+    w = rnd((ci, c, 2, 2, 2), torch.float32, 0.05)
+    wf = be.pack_weight(w, UP, "fwd", torch.bfloat16, 3, vox=s ** 3)
+    wd = be.pack_weight(w, UP, "dgrad", torch.bfloat16, 3, vox=sc ** 3)
+    bias = rnd((c,), torch.float32, 0.1)
+    y = torch.empty((n, s, s, s, c), dtype=torch.bfloat16, device=DEV)
+    stats = torch.zeros((n, c, 2), dtype=torch.float64, device=DEV)
+    be.conv(UP, 3, x, wf, bias, y, stats, None)
+    gamma, beta = rnd((c,), torch.float32) + 1.0, rnd((c,), torch.float32, 0.1)
+    scale = torch.full((n, c), 1.25, dtype=torch.float32, device=DEV)
+    gn = (stats, gamma, beta, scale, s ** 3, 8, 1e-5)
+    cat = torch.empty((n, s, s, s, 2 * c), dtype=torch.bfloat16, device=DEV)
+    gcat = rnd((n, s, s, s, 2 * c))
+    sums = torch.zeros((n, c, 3), dtype=torch.float64, device=DEV)
+    dy = torch.empty_like(y)
+    dx = torch.empty_like(x)
+    dwp = torch.zeros((8, c, ci), dtype=torch.float32, device=DEV)
+    d16 = [torch.zeros(c, device=DEV) for _ in range(3)]
+    tm.run(f"conv[k{UP}]   (UP)      {ci}->{c} @{sc}^3", lambda: be.conv(UP, 3, x, wf, bias, y, stats, None),
+           bytes_=X + T)
+    tm.run(f"apply_gn     -> cat[:16] C={c} @{s}^3", lambda: be.apply_gn(y, gn, None, None, None, cat[..., :c]),
+           bytes_=2 * T)
+    tm.run(f"gn_bwd_reduce_gn gcat[:16] C={c} @{s}^3", lambda: be.gn_bwd_reduce_gn(gcat[..., :c], y, gn, sums),
+           bytes_=2 * T)
+    tm.run(f"gn_bwd_apply_gn  gcat[:16] C={c} @{s}^3",
+           lambda: be.gn_bwd_apply_gn(gcat[..., :c], y, gn, sums, dy, *d16), bytes_=3 * T)
+    tm.run(f"wgrad[k{DOWN}]  (DOWN)    {c}x{ci} @{s}^3", lambda: be.wgrad(DOWN, 3, dy, x, dwp), bytes_=T + X)
+    tm.run(f"conv[k{DOWN}]   (dgrad)   {c}->{ci} @{s}^3", lambda: be.conv(DOWN, 3, dy, wd, None, dx, None, None),
+           bytes_=T + X)
+    g16 = rnd((n, s, s, s, c))
+    tm.run(f"gn_bwd_reduce_gn (ops.0) C={c} @{s}^3", lambda: be.gn_bwd_reduce_gn(g16, y, gn, sums), bytes_=2 * T)
+    if not hasattr(be, "up_gn_ok") or not be.up_gn_ok(x, wf, c, 3):
+        return
+    # the four fused launches that replace the first six (csrc/up_gn.cu)
+    tm.run(f"up_gn_stats         {ci}->{c} @{sc}^3", lambda: be.up_gn_stats(x, wf, bias, stats), bytes_=X)
+    tm.run(f"up_gn_apply         {ci}->{c} @{sc}^3", lambda: be.up_gn_apply(x, wf, bias, gn, cat[..., :c]),
+           bytes_=X + T)
+    tm.run(f"up_gn_bwd_sums      {ci}->{c} @{sc}^3", lambda: be.up_gn_bwd_sums(x, wf, bias, gn, gcat[..., :c], sums),
+           bytes_=X + T)
+    tm.run(f"up_gn_bwd           {ci}->{c} @{sc}^3",
+           lambda: be.up_gn_bwd(x, wf, bias, gn, gcat[..., :c], sums, dwp, dx, *d16), bytes_=2 * X + T,
+           flops=2 * n * s ** 3 * c * ci * 3)
+
+
 def bench_gn(be, tm, n):
     for c, s in ((16, 96), (32, 96), (32, 48), (64, 24), (128, 12), (256, 6)):
         vox = s ** 3
@@ -244,7 +294,7 @@ def bench_convbwd(be, tm, n):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=7)
-    ap.add_argument("--only", default="stem,stemgn,gn,pack,wgrad,conv")
+    ap.add_argument("--only", default="stem,stemgn,up,gn,pack,wgrad,conv")
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--tag", default="run")
     ap.add_argument("--eager", action="store_true", help="launch every op twice without graphs/timing (ncu runs)")
@@ -257,6 +307,8 @@ def main():
             bench_stem(be, tm, a.batch, 96)
         if "stemgn" in which:
             bench_stem_gn(be, tm, a.batch, 96)
+        if "up" in which:
+            bench_up(be, tm, a.batch)
         if "gn" in which:
             bench_gn(be, tm, a.batch)
         if "pack" in which:
