@@ -66,6 +66,9 @@ extern "C" {
 #define B200SEG_CONV_STEM 6      /* stem.cu: one input channel on CUDA cores */
 #define B200SEG_CONV_SMALLCIN 7  /* small_channels.cu: <= 4 input channels */
 #define B200SEG_CONV_GENERIC 8   /* conv_generic.cu: any shape */
+/* output tile geometries of B200SEG_CONV_HALO_WS (b200seg_conv_halo_ws_geometry) */
+#define B200SEG_WS_GEOM_COLUMN 0 /* 8 wide x 16 high tiles of the H x W plane */
+#define B200SEG_WS_GEOM_FLAT 1   /* 128 consecutive anchors h * (W + 2) + w of the padded plane */
 /* kernel families b200seg_wgrad chooses from (b200seg_wgrad_path) */
 #define B200SEG_WGRAD_HALO_MMA 0 /* wgrad_halo_mma.cu: 3x3x3, 16/32 channels, >= 32768 voxels */
 #define B200SEG_WGRAD_TC 1       /* wgrad_tc.cu: wgmma + TMA */
@@ -145,6 +148,10 @@ int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, i
  * B200SEG_EINVAL where b200seg_conv would refuse them */
 int b200seg_conv_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                       const b200seg_tensor* addend);
+/* the B200SEG_WS_GEOM_* output tile geometry b200seg_conv / b200seg_conv_bwdstats would use for these arguments on
+ * the B200SEG_CONV_HALO_WS path (chosen by the plane's shape; host only), or B200SEG_EINVAL if they take another path */
+int b200seg_conv_halo_ws_geometry(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
+                                  const b200seg_tensor* addend);
 
 /* Data-gradient convolution that ALSO accumulates the GroupNorm-backward sums of the layer behind its output:
  * g = conv_kind(x, wpk) [+ addend] is dL/d(activation) of the layer whose raw conv output is `yfwd` and whose

@@ -22,6 +22,8 @@ NORM_NONE, NORM_MEANSTD, NORM_PCTL = 0, 1, 2
 # kernel families of b200seg_conv / b200seg_wgrad (include/b200seg.h: B200SEG_CONV_*, B200SEG_WGRAD_*)
 CONV_PATHS = ("PW_MMA", "TC", "HALO2D", "HALO3", "HALO_WS", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
 WGRAD_PATHS = ("HALO_MMA", "TC", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
+# output tile geometries of the HALO_WS family (B200SEG_WS_GEOM_*): 8 x 16 column tiles, flattened padded rows
+HALO_WS_GEOMS = ("COLUMN", "FLAT")
 # voxels per sample a 3x3x3 layer needs before its weights are packed for the halo-staged kernels (16/32 channels)
 # and the weight-streaming halo kernel (64/128 channels); smaller layers take the TMA implicit-GEMM kernel
 HALO_MIN_VOX = 128 * 128
@@ -62,6 +64,7 @@ _SIGNATURES = {
     "b200seg_upload_table": ([_vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_conv": ([_i, _i, _PT, _vp, _i, _vp, _PT, _vp, _PT, _i, _vp], C.c_int),
     "b200seg_conv_path": ([_i, _i, _PT, _i, _PT, _PT], C.c_int),
+    "b200seg_conv_halo_ws_geometry": ([_i, _i, _PT, _i, _PT, _PT], C.c_int),
     "b200seg_conv_bwdstats_supported": ([_i, _i, _PT, _i, _PT, _PT, _PT], C.c_int),
     "b200seg_conv_bwdstats": ([_i, _i, _PT, _vp, _i, _PT, _PT, _PT, _PG, _vp, _i, _vp], C.c_int),
     "b200seg_conv_tc_eligible": ([_i, _i, _i], C.c_int),
@@ -413,6 +416,16 @@ class CudaBackend:
         if rc < 0:
             raise RuntimeError(f"libb200seg error {rc}: {self.lib.b200seg_last_error().decode()}")
         return CONV_PATHS[rc]
+
+    def conv_halo_ws_geometry(self, kind, dims, x, wpk, y, addend=None):
+        """output tile geometry (HALO_WS_GEOMS) the HALO_WS kernel family would use for these arguments; raises where
+        ``conv`` would take another family; launches nothing"""
+        code = BF16 if self._needs_repack(wpk, x, y) else wpk.code
+        dx, dy, da = _desc(x), _desc(y), _desc(addend)
+        rc = self.lib.b200seg_conv_halo_ws_geometry(kind, dims, C.byref(dx), code, C.byref(dy), _ref(da))
+        if rc < 0:
+            raise RuntimeError(f"libb200seg error {rc}: {self.lib.b200seg_last_error().decode()}")
+        return HALO_WS_GEOMS[rc]
 
     def wgrad_path(self, kind, dims, a, b):
         """name (WGRAD_PATHS) of the kernel family ``wgrad`` would launch for these arguments; launches nothing"""

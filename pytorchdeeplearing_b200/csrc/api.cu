@@ -34,6 +34,7 @@ int pw_mma_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, c
 int pw_mma_conv(int kind, int dims, const b200seg_tensor* x, const void* w, const float* bias,
                 const b200seg_tensor* y, double* stats, const b200seg_tensor* addend, int device, cudaStream_t st);
 int conv_halows_ntile(int kind, int cin, int cout);
+int conv_halows_geometry(int cin, int h, int w);
 int conv_halows_supported(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
                           const b200seg_tensor* addend);
 int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, const float* bias,
@@ -263,6 +264,17 @@ int b200seg_conv_path(int kind, int dims, const b200seg_tensor* x, int w_dtype, 
   B200_CHECK_ARG(path >= 0, "b200seg_conv_path: packed tensor-core weights need bf16, 16-byte aligned activations of "
                  "a supported shape");
   return path;
+}
+
+int b200seg_conv_halo_ws_geometry(int kind, int dims, const b200seg_tensor* x, int w_dtype, const b200seg_tensor* y,
+                                  const b200seg_tensor* addend) {
+  REQ_TENSOR(x, "x");
+  REQ_TENSOR(y, "y");
+  OPT_TENSOR(addend, "addend");
+  B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_conv_halo_ws_geometry: dims must be 2 or 3");
+  B200_CHECK_ARG(conv_path(kind, dims, x, w_dtype, y, addend) == B200SEG_CONV_HALO_WS,
+                 "b200seg_conv_halo_ws_geometry: these arguments do not take the weight-streaming halo kernel");
+  return conv_halows_geometry(x->c, x->h, x->w);   // what conv_halows itself switches on
 }
 
 int b200seg_conv(int kind, int dims, const b200seg_tensor* x, const void* wpk, int w_dtype, const float* bias,

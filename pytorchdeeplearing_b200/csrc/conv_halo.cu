@@ -278,23 +278,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_kernel(const HaloAr
               s[j] = valid ? v[j] : 0.f;
               qq[j] = s[j] * s[j];
             }
-#pragma unroll
-            for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-              const bool up = (lane & off) != 0;
-#pragma unroll
-              for (int j = 0; j < half; ++j) {
-                const float keep_s = up ? s[j + half] : s[j];
-                const float send_s = up ? s[j] : s[j + half];
-                const float keep_q = up ? qq[j + half] : qq[j];
-                const float send_q = up ? qq[j] : qq[j + half];
-                s[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-                qq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-              }
-            }
-            s[0] += __shfl_xor_sync(0xffffffffu, s[0], 1);
-            qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
+            stat_butterfly(s, qq, lane);
             if ((lane & 1) == 0) {
-              const int col = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
+              const int col = stat_col(lane);
               // this lane is the only writer of its column in this warp's private row: no atomics, fixed order
               float* sw_ = s_stat + q * 2 * p.Cout;
               sw_[c0 + col] += s[0];
@@ -772,23 +758,9 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
             s[j] = rs[c0 + j];
             qq[j] = rq[c0 + j];
           }
-#pragma unroll
-          for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-            const bool up = (lane & off) != 0;
-#pragma unroll
-            for (int j = 0; j < half; ++j) {
-              const float keep_s = up ? s[j + half] : s[j];
-              const float send_s = up ? s[j] : s[j + half];
-              const float keep_q = up ? qq[j + half] : qq[j];
-              const float send_q = up ? qq[j] : qq[j + half];
-              s[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-              qq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-            }
-          }
-          s[0] += __shfl_xor_sync(0xffffffffu, s[0], 1);
-          qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
+          stat_butterfly(s, qq, lane);
           if ((lane & 1) == 0) {
-            const int col = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
+            const int col = stat_col(lane);
             float* sw_ = s_stat + (warp - 4) * 2 * p.Cout;   // this warp's private row: no atomics, fixed order
             sw_[c0 + col] += s[0];
             sw_[p.Cout + c0 + col] += qq[0];

@@ -9,10 +9,21 @@
 //   * weights: the 27 tap blocks ([Cin/8][NT][8] bf16, 8-16 KB) of an output-channel group are too large to stay
 //     resident beside the slices, so they are streamed through a cp.async.bulk ring (as deep as the shared memory
 //     left over allows: the blocks in flight hide the L2 latency of the stream).
-// Work split: the output space is T = N * th * tw * (Cout / NT) * D units, one (8 x 16 slice tile, NT-channel group)
-// each, ordered (n, h tile, w tile, group, d).  CTA b of G owns [b*T/G, (b+1)*T/G) and walks it as column segments
-// (n, h0, w0, group, d_a, nd); every role takes its segments from ws_segment, so their slice, tap-block and output
-// sequences, and with them the mbarrier parities, agree.  A segment stages its input slices d_a-1 .. d_a+nd once.
+// Output tile geometry (M = 128 rows), chosen per launch by shape (conv_halows_geometry):
+//   * column: 8 wide x 16 high.  One core matrix is one 8-voxel output row, so the tile covers a plane exactly only
+//     where 8 | W and 16 | H (UNet3d's 32^2 / 16^2 planes); 128 input channels always use it;
+//   * flattened padded rows: with P = W + 2 the padded row pitch, output (h, w) is anchor position q = h*P + w and
+//     tap (kh, kw) reads padded position q + kh*P + kw, one constant offset over a run of consecutive positions.  A
+//     tile is 128 consecutive anchors [q0, q0 + 128); its slice window is padded positions [q0, q0 + 128 + 2P + 2)
+//     (SBO = 16 B x 8 positions).  The two wrap-around anchors per padded row (w = W, W + 1) are computed and
+//     dropped by the epilogue.  A 24 x 24 plane takes 5 such tiles (640 rows) instead of 2 x 3 column tiles (768),
+//     and a tile whose upper M64 half lies wholly past the last anchor issues only its lower half's MMAs.
+//   Both read the same packed weights in the same (kd, kh, kw, kc) order: every output value is the same in either.
+// Work split: the output space is T = N * th * tw * (Cout / NT) * D units, one (slice tile, NT-channel group)
+// each, ordered (n, h tile, w tile, group, d) (flat: th = tiles, tw = 1).  CTA b of G owns [b*T/G, (b+1)*T/G) and
+// walks it as column segments (n, tile, group, d_a, nd); every role takes its segments from ws_segment, so their
+// slice, tap-block and output sequences, and with them the mbarrier parities, agree.  A segment stages its input
+// slices d_a-1 .. d_a+nd once.
 //   * items: a segment is cut into items of NACC consecutive output slices (the last one may be shorter).  Each
 //     streamed tap block is multiplied into all of the item's accumulators (registers of the MMA warpgroup), so the
 //     weight traffic per output tile drops by NACC.  Every output sums its 27 taps x Cin/16 K chunks in the order
@@ -37,8 +48,12 @@
 
 namespace b200seg {
 
-constexpr int WS_TW = 8, WS_TH = 16;                 // output tile (w, h); M = 128 rows = (hh, ww)
+constexpr int WS_TW = 8, WS_TH = 16;                 // column output tile (w, h); M = 128 rows = (hh, ww)
 constexpr int WS_PW = WS_TW + 2, WS_PH = WS_TH + 2;
+constexpr int WS_M = WS_TW * WS_TH;                  // output rows per tile (both geometries)
+// flat tiles are used only while their slice window (128 + 2P + 2 positions) is no longer than 184 positions (W <= 25),
+// about the column window's 18 x 10 = 180: the shared-memory split of conv_halows_launch stays what it was
+constexpr int kWsFlatMaxPos = 184;
 constexpr int kWsMaxSlices = 8;
 constexpr int kWsSliceLoaders = 3;                   // warps 8..10; warp 11 streams the weights
 constexpr int kWsThreads = 32 * (4 + 4 + 4);         // 384 threads
@@ -62,7 +77,10 @@ struct HaloWsArgs {
   long long xld, yld, ald;
   int N, D, H, W;
   int Cin, Cout;
-  int tw, th;             // tiles along w, h
+  int tw, th;             // tiles along w, h (flat: tw = 1, th = tiles of 128 anchors)
+  int P;                  // flat: padded row pitch W + 2
+  int span;               // flat: anchors of a plane, (H - 1) * P + W
+  int npos;               // positions of one staged slice plane (flat: 128 + 2P + 2, column: 18 x 10)
   int ngroups;            // output-channel groups of NT columns
   int nslices;            // input slice ring size (>= NACC + 2)
   int wstages;            // weight ring depth (tap blocks in flight)
@@ -91,9 +109,10 @@ __device__ __forceinline__ void ws_range(const HaloWsArgs& p, int& begin, int& e
   end = (int)(nunits * (blockIdx.x + 1) / gridDim.x);
 }
 
-// one column segment of a CTA's range: nd output slices from (n, d0) of the (h0, w0) column, channel group g
+// one column segment of a CTA's range: nd output slices from (n, d0) of the (h0, w0) column (flat: of the tile whose
+// first anchor is q0), channel group g
 struct WsSeg {
-  int n, h0, w0, g, d0, nd;
+  int n, h0, w0, q0, g, d0, nd;
 };
 // the segment starting at unit u of a CTA range that ends at `end` (units ordered (n, h tile, w tile, group, d))
 __device__ __forceinline__ WsSeg ws_segment(const HaloWsArgs& p, int u, int end) {
@@ -108,16 +127,18 @@ __device__ __forceinline__ WsSeg ws_segment(const HaloWsArgs& p, int u, int end)
   s.n = c / p.th;
   s.w0 = iw * WS_TW;
   s.h0 = ih * WS_TH;
+  s.q0 = ih * WS_M;
   s.nd = min(p.D - s.d0, end - u);
   return s;
 }
 
-template <int CIN, int NT, int NACC, bool BWD>
+template <int CIN, int NT, int NACC, bool BWD, bool FLAT>
 __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWsArgs p) {
   PDL_TRIGGER();
   constexpr int CP = CIN / 8;                                // 8-channel planes
-  constexpr uint32_t PLANE = WS_PH * WS_PW * 16u;            // bytes of one plane of one slice
-  constexpr uint32_t SLICE = (uint32_t)CP * PLANE;
+  const int npos = FLAT ? p.npos : WS_PH * WS_PW;            // positions of one plane of one slice
+  const uint32_t PLANE = (uint32_t)npos * 16u;               // bytes of one plane of one slice
+  const uint32_t SLICE = (uint32_t)CP * PLANE;
   constexpr int TAPS = 27;
   constexpr uint32_t TAP_BYTES = (uint32_t)CIN * NT * 2u;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -171,7 +192,11 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     // ===================================================== MMA warpgroup
     setmaxnreg_inc<kWsRegsMma>();
     const int wt = threadIdx.x;
-    const uint64_t a_hi = ws_nosw_desc(PLANE, WS_PW * 16u);
+    // column: one core matrix = one 8-voxel halo row (SBO = one halo row); flat: 8 consecutive positions (SBO = 128 B)
+    const uint64_t a_hi = ws_nosw_desc(PLANE, FLAT ? 128u : WS_PW * 16u);
+    const uint32_t pitch = FLAT ? (uint32_t)p.P : (uint32_t)WS_PW;   // positions from one kh to the next
+    // rows 64..127 of the tile: 8 halo rows further on (column), 64 positions further on (flat)
+    constexpr uint32_t hi_off = (FLAT ? 64u * 16u : 8u * WS_PW * 16u) >> 4;
     const uint64_t b_hi = ws_nosw_desc((uint32_t)NT * 16u, 128u);
     const uint32_t ring_u32 = smem_u32(s_ring);
     const uint32_t w_u32 = smem_u32(s_w);
@@ -189,12 +214,17 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
     };
     for (int u = u_begin; u < u_end;) {
       const WsSeg s = ws_segment(p, u, u_end);
+      // a flat tile whose upper M64 half lies wholly past the plane's last anchor computes its lower half only (its
+      // upper accumulators stay zero and the epilogue drops those rows)
+      const bool upper = !FLAT || s.q0 + 64 < p.span;
       for (int o0 = 0; o0 < s.nd; o0 += NACC) {
         const bool last = o0 + NACC >= s.nd;       // last item of the segment
         const uint32_t f = gs + (uint32_t)o0;      // ring position of the item's first input slice
         // one item of NA output slices: reads input slices f .. f + NA + 1, output j and tap kd read slice f + j + kd
-        auto item = [&](auto na_) {
+        auto item = [&](auto na_, auto up_) {
           constexpr int NA = decltype(na_)::value;
+          constexpr bool UP = decltype(up_)::value;   // the upper M64 half is computed (a compile-time choice: a
+                                                      // branch inside the chain would make ptxas serialise the wgmmas)
           float acc[NA][2][NT / 2];
 #pragma unroll
           for (int j = 0; j < NA; ++j) {
@@ -229,11 +259,10 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
                 const uint64_t a_base = a_hi | (uint64_t)((ring_u32 + (sl % ns) * SLICE) >> 4);
 #pragma unroll
                 for (int kc = 0; kc < kchunks; ++kc) {
-                  const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + (uint32_t)((t9 / 3) * WS_PW + t9 % 3) * 16u) >> 4;
+                  const uint32_t a_off = ((uint32_t)(2 * kc) * PLANE + ((uint32_t)(t9 / 3) * pitch + t9 % 3) * 16u) >> 4;
                   const uint32_t b_off = ((uint32_t)(kc * 2 * NT) * 16u) >> 4;
                   Wgmma<NT, 0, 0>::mma(acc[j][0], a_base + a_off, b_tap + b_off);
-                  // rows 64..127 of the tile (hh = 8..15) start 8 halo rows further on
-                  Wgmma<NT, 0, 0>::mma(acc[j][1], a_base + a_off + (8u * WS_PW * 16u >> 4), b_tap + b_off);
+                  if constexpr (UP) Wgmma<NT, 0, 0>::mma(acc[j][1], a_base + a_off + hi_off, b_tap + b_off);
                 }
               }
               wgmma_commit();
@@ -274,8 +303,12 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
           }
           go += (uint32_t)NA;
         };
-        if (o0 + NACC <= s.nd) item(std::integral_constant<int, NACC>{});
-        else item(std::integral_constant<int, 1>{});   // NACC = 2: the odd last slice of a segment
+        auto halves = [&](auto up_) {
+          if (o0 + NACC <= s.nd) item(std::integral_constant<int, NACC>{}, up_);
+          else item(std::integral_constant<int, 1>{}, up_);   // NACC = 2: the odd last slice of a segment
+        };
+        if (upper) halves(std::true_type{});
+        else if constexpr (FLAT) halves(std::false_type{});
       }
       gs += (uint32_t)(s.nd + 2);
       u += s.nd;
@@ -312,9 +345,9 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       // takes its next one: the ring may hold just one item's NACC + 2 slices, and the slot of a later slice is only
       // freed once the MMA warpgroup has read this one.
       const int lw = warp - 8;
-      constexpr int pieces = WS_PH * WS_PW * CP;
+      const int pieces = npos * CP;
       int u = u_begin, it_i = 0, it_nsl = 0;
-      WsSeg s{0, 0, 0, 0, 0, 0};
+      WsSeg s{0, 0, 0, 0, 0, 0, 0};
       auto load_seg = [&]() {
         if (u < u_end) {
           s = ws_segment(p, u, u_end);
@@ -339,16 +372,40 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
         const int d = s.d0 - 1 + it_i;
         const bool dok = (unsigned)d < (unsigned)p.D;
         const bf16* src = p.x + (((long long)s.n * p.D + (dok ? d : 0)) * p.H) * p.W * p.xld;
+        if constexpr (FLAT) {
+          // a lane keeps one 8-channel plane (32 % CP == 0) and walks positions v = lane / CP + k * 32 / CP; padded
+          // position q0 + v = (hp, wp) holds source voxel (hp - 1, wp - 1), stepped without a division per piece
+          constexpr int VSTEP = 32 / CP;
+          const int plane = lane % CP;
+          int v = lane / CP;
+          int hp = (int)((unsigned)(s.q0 + v) / (unsigned)p.P);
+          int wp = s.q0 + v - hp * p.P;
 #pragma unroll 4
-        for (int q = lane; q < pieces; q += 32) {
-          const int v = q / CP, plane = q - v * CP;
-          const int hh = v / WS_PW, ww = v - hh * WS_PW;
-          const int h = s.h0 - 1 + hh, w = s.w0 - 1 + ww;
-          const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
-          const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
-                       "l"(g), "r"(ok ? 16 : 0)
-                       : "memory");
+          for (; v < npos; v += VSTEP) {
+            const int h = hp - 1, w = wp - 1;
+            const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
+            const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
+                         "l"(g), "r"(ok ? 16 : 0)
+                         : "memory");
+            wp += VSTEP;
+            while (wp >= p.P) {
+              wp -= p.P;
+              ++hp;
+            }
+          }
+        } else {
+#pragma unroll 4
+          for (int q = lane; q < pieces; q += 32) {
+            const int v = q / CP, plane = q - v * CP;
+            const int hh = v / WS_PW, ww = v - hh * WS_PW;
+            const int h = s.h0 - 1 + hh, w = s.w0 - 1 + ww;
+            const bool ok = dok && (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
+            const bf16* g = ok ? src + ((long long)h * p.W + w) * p.xld + plane * 8 : p.x;
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(plane * (int)PLANE + v * 16)),
+                         "l"(g), "r"(ok ? 16 : 0)
+                         : "memory");
+          }
         }
         asm volatile("cp.async.wait_all;" ::: "memory");
         fence_proxy_async();            // landed cp.async data -> visible to the tensor core (async proxy)
@@ -429,7 +486,13 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
         cur_n = n;
         if constexpr (BWD) load_coefs(n);
       }
-      const int oh = sg.h0 + rh, ow = sg.w0 + rw;
+      int oh = sg.h0 + rh, ow = sg.w0 + rw;
+      if constexpr (FLAT) {
+        // anchor q = oh * P + ow; the wrap-around anchors (ow = W, W + 1) and those past the plane are not outputs
+        const int qa = sg.q0 + row;
+        oh = (int)((unsigned)qa / (unsigned)p.P);
+        ow = qa - oh * p.P;
+      }
       const bool valid = oh < p.H && ow < p.W;
       const int cbase = sg.g * NT;
       float rs[NT], rq[NT];
@@ -526,23 +589,9 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
             s[j] = rs[c * 16 + j];
             qq[j] = rq[c * 16 + j];
           }
-#pragma unroll
-          for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-            const bool up = (lane & off) != 0;
-#pragma unroll
-            for (int j = 0; j < half; ++j) {
-              const float keep_s = up ? s[j + half] : s[j];
-              const float send_s = up ? s[j] : s[j + half];
-              const float keep_q = up ? qq[j + half] : qq[j];
-              const float send_q = up ? qq[j] : qq[j + half];
-              s[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-              qq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-            }
-          }
-          s[0] += __shfl_xor_sync(0xffffffffu, s[0], 1);
-          qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
+          stat_butterfly(s, qq, lane);
           if ((lane & 1) == 0) {
-            const int col = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
+            const int col = stat_col(lane);
             float* sw_ = s_stat + q * 2 * p.Cout;     // this warp's private row: no atomics, fixed order
             sw_[cbase + c * 16 + col] += s[0];
             sw_[p.Cout + cbase + c * 16 + col] += qq[0];
@@ -577,12 +626,40 @@ int conv_halows_supported(int kind, int dims, const b200seg_tensor* x, int w_dty
   return 1;
 }
 
+// The output tile geometry of a layer with Cin input channels and an H x W plane: flattened padded rows at 64 input
+// channels where they need fewer tiles per plane than the 8 x 16 column tile and their slice window fits the
+// column's shared-memory budget; a tie keeps the column tile.  Fewer tiles means fewer units, and so fewer per CTA:
+// 24 x 24 takes 5 flat tiles instead of 6 (64 -> 64 at 2 x 24^3 on an H100: 31.5 -> 29.5 us forward, 39.6 -> 35.6 us
+// for the data gradient with GroupNorm-backward sums).  Fewer MMA rows alone do not pay: at 12 x 12 the flat split is
+// one full tile and one lower-half tile, two units per (n, d, group) as with two column tiles, and a trial of it at
+// 128 channels measured no faster, so 128 input channels and the planes the column tile covers exactly (8 | W,
+// 16 | H) stay on the column tile.
+// Where flat is chosen no CTA gets more units than under the column split.  b200seg_conv_halo_ws_geometry reports
+// this same value.
+int conv_halows_geometry(int cin, int h, int w) {
+  if (cin != 64) return B200SEG_WS_GEOM_COLUMN;
+  const long long col_tiles = (long long)((h + WS_TH - 1) / WS_TH) * ((w + WS_TW - 1) / WS_TW);
+  const int P = w + 2;
+  if (WS_M + 2 * P + 2 > kWsFlatMaxPos) return B200SEG_WS_GEOM_COLUMN;
+  const long long flat_tiles = ((long long)(h - 1) * P + w + WS_M - 1) / WS_M;
+  return flat_tiles < col_tiles ? B200SEG_WS_GEOM_FLAT : B200SEG_WS_GEOM_COLUMN;
+}
+
 static int g_ws_init[64] = {0};
 
+template <int CIN, int NT, int NACC, bool FLAT>
+static int conv_halows_set_smem(int maxsm) {
+  B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<CIN, NT, NACC, false, FLAT>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<CIN, NT, NACC, true, FLAT>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+  return B200SEG_OK;
+}
+
 template <int CIN, int NT, int NACC>
-static int conv_halows_launch(HaloWsArgs& p, int device, int maxsm, cudaStream_t st) {
+static int conv_halows_launch(HaloWsArgs& p, int flat, int device, int maxsm, cudaStream_t st) {
   // (tail: barriers, statistics rows, bias, the A/B table and its fp64 scratch for the backward-sums epilogue)
-  const int slice = (CIN / 8) * WS_PH * WS_PW * 16;
+  const int slice = (CIN / 8) * p.npos * 16;
   const int tap_bytes = CIN * NT * 2;
   const int tail0 = (2 * kWsMaxSlices + 4 + 2 * kWsMaxWStages) * 8 + 16 + 11 * p.Cout * 4 + 64 +
                     (2 * p.Cout + 16) * 8 + 8 + 16;
@@ -607,12 +684,24 @@ static int conv_halows_launch(HaloWsArgs& p, int device, int maxsm, cudaStream_t
   p.ngroups = p.Cout / NT;
   const size_t smem_bytes = 128 + (size_t)wst * tap_bytes + (size_t)ns * slice + (size_t)tail0 +
                             128u * (size_t)p.acc_pitch * 4u;
-  // the N * th * tw * ngroups * D units are split evenly over at most one CTA per SM
+  // the N * th * tw * ngroups * D units are split evenly over at most one CTA per SM.  Flat tiles take just enough
+  // CTAs for the largest share, ceil(units / SMs): 240 units at 2 x 24^3 go two to each of 120 CTAs, so with an even
+  // D every CTA's pair is one NACC = 2 item of one column (one weight stream), where 132 CTAs would leave some pairs
+  // split across two columns.  The largest share, and so the statistics fold count per CTA, is the same either way.
   const long long nunits = (long long)p.N * p.th * p.tw * p.ngroups * p.D;
   const int sms = num_sms(device);
-  const int grid = nunits < sms ? (int)nunits : sms;
-  if (p.yfwd != nullptr) launch_k(conv_halows_kernel<CIN, NT, NACC, true>, grid, kWsThreads, smem_bytes, st, p);
-  else launch_k(conv_halows_kernel<CIN, NT, NACC, false>, grid, kWsThreads, smem_bytes, st, p);
+  int grid = nunits < sms ? (int)nunits : sms;
+  if (flat) {
+    const long long share = (nunits + grid - 1) / grid;
+    grid = (int)((nunits + share - 1) / share);
+  }
+  if (flat) {
+    if (p.yfwd != nullptr) launch_k(conv_halows_kernel<CIN, NT, NACC, true, true>, grid, kWsThreads, smem_bytes, st, p);
+    else launch_k(conv_halows_kernel<CIN, NT, NACC, false, true>, grid, kWsThreads, smem_bytes, st, p);
+  } else {
+    if (p.yfwd != nullptr) launch_k(conv_halows_kernel<CIN, NT, NACC, true, false>, grid, kWsThreads, smem_bytes, st, p);
+    else launch_k(conv_halows_kernel<CIN, NT, NACC, false, false>, grid, kWsThreads, smem_bytes, st, p);
+  }
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }
@@ -623,10 +712,11 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
   (void)kind; (void)dims;
   const int maxsm = tc_max_smem(device);
   if (device >= 0 && device < 64 && !g_ws_init[device]) {
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<128, 64, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<64, 64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
-    B200_CUDA(cudaFuncSetAttribute(conv_halows_kernel<128, 64, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsm));
+    if (conv_halows_set_smem<64, 64, 2, false>(maxsm) != B200SEG_OK ||
+        conv_halows_set_smem<128, 64, 1, false>(maxsm) != B200SEG_OK ||
+        conv_halows_set_smem<64, 64, 2, true>(maxsm) != B200SEG_OK ||
+        conv_halows_set_smem<128, 64, 1, true>(maxsm) != B200SEG_OK)
+      return B200SEG_ECUDA;
     g_ws_init[device] = 1;
   }
   HaloWsArgs p;
@@ -639,8 +729,20 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
   p.xld = x->ld; p.yld = y->ld; p.ald = addend ? addend->ld : 0;
   p.N = x->n; p.D = x->d; p.H = x->h; p.W = x->w;
   p.Cin = x->c; p.Cout = y->c;
-  p.tw = (p.W + WS_TW - 1) / WS_TW;
-  p.th = (p.H + WS_TH - 1) / WS_TH;
+  const int flat = conv_halows_geometry(p.Cin, p.H, p.W) == B200SEG_WS_GEOM_FLAT;
+  if (flat) {
+    p.P = p.W + 2;
+    p.span = (p.H - 1) * p.P + p.W;
+    p.npos = WS_M + 2 * p.P + 2;
+    p.tw = 1;
+    p.th = (p.span + WS_M - 1) / WS_M;
+  } else {
+    p.P = 0;
+    p.span = 0;
+    p.npos = WS_PH * WS_PW;
+    p.tw = (p.W + WS_TW - 1) / WS_TW;
+    p.th = (p.H + WS_TH - 1) / WS_TH;
+  }
   p.yfwd = nullptr; p.yfld = 0; p.gstats = nullptr; p.ggamma = nullptr; p.gbeta = nullptr; p.gscale = nullptr;
   p.ggroups = 1; p.gm = 1.0; p.geps = 0.f;
   if (yfwd != nullptr) {
@@ -658,8 +760,8 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
   }
   // NT = 64 columns per MMA (narrower groups re-read A for less work).  Two output slices share each streamed tap
   // block at 64 input channels; at 128 the four input slices that takes do not fit beside the staging tile.
-  if (p.Cin == 64) return conv_halows_launch<64, 64, 2>(p, device, maxsm, st);
-  return conv_halows_launch<128, 64, 1>(p, device, maxsm, st);
+  if (p.Cin == 64) return conv_halows_launch<64, 64, 2>(p, flat, device, maxsm, st);
+  return conv_halows_launch<128, 64, 1>(p, flat, device, maxsm, st);
 }
 
 }  // namespace b200seg

@@ -80,29 +80,7 @@ constexpr int kTcThreads = 256 + 32 * kEpiWarps * kEpiGroups;
 constexpr int kMaxAcc = 2;            // accumulator staging slots (one per epilogue group)
 constexpr int kTcMaxN = 64;           // MMA N per tile: both M64 halves of the accumulator stay in registers
 
-// butterfly transpose-reduce of 16 per-lane column values (and their squares) over the 32 lanes of a warp:
-// afterwards every EVEN lane L holds in s[0] / q[0] the warp totals of column stat_col(L)
-__device__ __forceinline__ void stat_butterfly(float* s, float* qq, int lane) {
-#pragma unroll
-  for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int j = 0; j < half; ++j) {
-      const float keep_s = up ? s[j + half] : s[j];
-      const float send_s = up ? s[j] : s[j + half];
-      const float keep_q = up ? qq[j + half] : qq[j];
-      const float send_q = up ? qq[j] : qq[j + half];
-      s[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, off);
-      qq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, off);
-    }
-  }
-  s[0] += __shfl_xor_sync(0xffffffffu, s[0], 1);
-  qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
-}
-// column owned by an even lane after stat_butterfly: bit k of the index is bit (4-k) of the lane for k = 0..3
-__device__ __forceinline__ int stat_col(int lane) {
-  return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-}
+// stat_butterfly / stat_col: tc_common.cuh
 
 template <int BKC, int N>
 __device__ __forceinline__ void tc_mma_role(const TcArgs& p, const uint8_t* smem, uint32_t STAGE, uint64_t* full,

@@ -138,6 +138,42 @@ __device__ __forceinline__ void acc_ld16(const float* s, float* v) {
   }
 }
 
+// p ? a : b on values in registers.  Written as `up ? s[j + half] : s[j]` the compiler selects between the two
+// ADDRESSES, which puts the whole array in local memory (every butterfly step then a dependent store and load).
+__device__ __forceinline__ float sel_f32(bool p, float a, float b) {
+  float r;
+  asm("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %3, 0;\n\tselp.f32 %0, %1, %2, q;\n\t}"
+      : "=f"(r)
+      : "f"(a), "f"(b), "r"((unsigned)p));
+  return r;
+}
+// one butterfly step: lanes with bit 2*HALF set keep the upper HALF values and send the lower ones (a constant trip
+// count per step, so every index is a compile-time constant and s / qq stay in registers)
+template <int HALF>
+__device__ __forceinline__ void stat_butterfly_step(float* s, float* qq, int lane) {
+  const bool up = (lane & (2 * HALF)) != 0;
+#pragma unroll
+  for (int j = 0; j < HALF; ++j) {
+    const float lo_s = s[j], hi_s = s[j + HALF], lo_q = qq[j], hi_q = qq[j + HALF];
+    s[j] = sel_f32(up, hi_s, lo_s) + __shfl_xor_sync(0xffffffffu, sel_f32(up, lo_s, hi_s), 2 * HALF);
+    qq[j] = sel_f32(up, hi_q, lo_q) + __shfl_xor_sync(0xffffffffu, sel_f32(up, lo_q, hi_q), 2 * HALF);
+  }
+}
+// butterfly transpose-reduce of 16 per-lane column values (and their squares) over the 32 lanes of a warp:
+// afterwards every EVEN lane L holds in s[0] / q[0] the warp totals of column stat_col(L)
+__device__ __forceinline__ void stat_butterfly(float* s, float* qq, int lane) {
+  stat_butterfly_step<8>(s, qq, lane);
+  stat_butterfly_step<4>(s, qq, lane);
+  stat_butterfly_step<2>(s, qq, lane);
+  stat_butterfly_step<1>(s, qq, lane);
+  s[0] += __shfl_xor_sync(0xffffffffu, s[0], 1);
+  qq[0] += __shfl_xor_sync(0xffffffffu, qq[0], 1);
+}
+// column owned by an even lane after stat_butterfly: bit k of the index is bit (4-k) of the lane for k = 0..3
+__device__ __forceinline__ int stat_col(int lane) {
+  return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
+}
+
 // Shared-memory matrix descriptors (layout type in bits 62-63: 1 = 128-byte, 2 = 64-byte, 3 = 32-byte swizzle).
 // K-major, swizzled operand tile (rows of `swizzle_bytes`, 8-row atoms): SBO = 8 * swizzle_bytes
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, uint32_t swizzle_bytes) {
