@@ -502,6 +502,27 @@ int b200seg_normalize(int norm_mode, const float* x, int oD, int oH, int oW, voi
 int b200seg_resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* ratio_zyx, int vD, int vH,
                                 int vW, int oD, int oH, int oW, uint8_t* out, int device, b200seg_stream stream);
 
+/* ---- 2-D image resize: OpenCV's uint8 cv2.resize(img, (oW, oH)) with the default INTER_LINEAR, as the reference's 2-D
+ * datasets (model/dataset.py:63,140,154: before the z-score; the segmentation label too) and 2-D inference methods
+ * (model/modelVNet.py:231-242,450-461, model/modelUnet.py:231-242,450-461, model/modelResNet.py:212-221,428-437: the
+ * image before "/ 255." and the uint8 mask back to image.shape) call it on the host.  Per axis (source size s,
+ * destination size d, destination index i): scale = 1.0 / ((double)d / s) in fp64; f = (float)((i + 0.5) * scale -
+ * 0.5) with the fp64 multiply and subtract rounded separately; k = floor(f), f -= k (fp32).  Along x, k < 0 gives
+ * k = 0, f = 0 and k >= s - 1 gives k = s - 1, f = 0, taps k and min(k + 1, s - 1); along y f is not clamped and the
+ * taps are clamp(k, 0, s - 1), clamp(k + 1, 0, s - 1).  c0 = rint((1 - f) * 2048), c1 = rint(f * 2048) (half to
+ * even).  Horizontal r = src[k] c0 + src[k + 1] c1 (int32); vertical, with b0, b1 the y coefficients and r0, r1 the
+ * two rows: v = (((b0 (r0 >> 4)) >> 16) + ((b1 (r1 >> 4)) >> 16) + 2) >> 2 (OpenCV's SIMD form, not the textbook
+ * (r0 b0 + r1 b1 + 2^21) >> 22), saturated to [0, 255].
+ * One launch resizes a ragged batch: desc (device memory, n entries) gives each sample's byte offset into src and its
+ * (h, w) >= 1, dense rows of w bytes.  out: dense [n][oH][oW], out_mode B200SEG_U8 (the cv2 bytes) or B200SEG_F32
+ * ((float)((double)v / 255.0): the inference methods' "/ 255." and .float()).  n <= 65535, sizes >= 1. */
+typedef struct b200seg_resize_src {
+  int64_t offset; /* byte offset of the sample's pixel (0, 0) in src */
+  int32_t h, w;   /* its height and width */
+} b200seg_resize_src;
+int b200seg_resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
+                             int out_mode, int device, b200seg_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

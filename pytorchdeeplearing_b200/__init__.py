@@ -5,7 +5,8 @@ Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-So
 3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``) and the SSIM losses of
 ``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``), and the whole-volume 3-D inference of
 ``XModel.inference`` / ``inference_patch`` with its resamples and normalisations (``inference3d``,
-``inference_patch3d``).
+``inference_patch3d``), and the 2-D ``XModel.inference`` and datasets' bit-exact cv2 bilinear resize (``inference2d``,
+``resize2d``, ``InputStager(max_source_pixels=...)``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -24,14 +25,14 @@ from .graphed import GraphedStep
 from .optim import FusedAdamW, FusedAdam
 from .metric import dice_coeff, iou_coeff, multiclass_dice_coeff, multiclass_iou_coeff, seg_metrics3d, Seg_Metirc3d
 from .inference import (predict, predict_mask, sliding_window_mask, inference3d, inference_patch3d, resample3d,
-                        spacing_size)
+                        spacing_size, resize2d, inference2d)
 from .staging import InputStager, stage_batch
 from .ssim import SSIM, SSIM3D, ssim, ssim3D
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
            "predict_mask",
-           "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d", "spacing_size", "InputStager", "stage_batch", "set_precision", "get_precision",
+           "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d", "spacing_size", "resize2d", "inference2d", "InputStager", "stage_batch", "set_precision", "get_precision",
            "enable_data_parallel", "disable_data_parallel", "install", "uninstall", "GraphedStep",
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import struct
 import threading
 from typing import Optional
 
@@ -134,6 +135,7 @@ _SIGNATURES = {
     "b200seg_resample_linear": ([_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _f, _f, _vp, _vp, _i64, _i, _vp], C.c_int),
     "b200seg_normalize": ([_i, _vp, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_resample_nearest_u8": ([_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp], C.c_int),
+    "b200seg_resize_linear_u8": ([_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -164,6 +166,14 @@ def load_library(path: Optional[str] = None):
         if path is None:
             _lib = lib
         return lib
+
+
+RESIZE_SRC_BYTES = 16      # sizeof(struct b200seg_resize_src)
+
+
+def resize_src_table(entries) -> bytes:
+    """[(byte offset, h, w)] of a ragged uint8 batch -> the host bytes of its ``b200seg_resize_src`` table"""
+    return b"".join(struct.pack("<qii", int(o), int(h), int(w)) for o, h, w in entries)
 
 
 def _dt(t: torch.Tensor) -> int:
@@ -941,6 +951,19 @@ class CudaBackend:
         r = (C.c_double * 3)(*[float(v) for v in ratio_zyx])
         self._check(self.lib.b200seg_resample_nearest_u8(src.data_ptr(), *src.shape, C.cast(r, _vp), *valid_zyx,
                                                          *out.shape, out.data_ptr(), dev, st))
+
+    # ------------------------------------------------------------------ 2-D image resize (csrc/resize2d.cu)
+    def resize_linear(self, src, desc, out):
+        """cv2.resize(INTER_LINEAR) of a ragged uint8 batch: src a uint8 device buffer holding every sample's rows,
+        desc int64 [N, 2] device: the bytes of ``resize_src_table`` (struct b200seg_resize_src), out dense
+        (N, oH, oW) uint8 (the cv2 bytes) or fp32 (v / 255)"""
+        dev, st = self._ds(src)
+        assert src.dtype == torch.uint8 and src.is_contiguous() and desc.dtype == torch.int64 and desc.is_contiguous()
+        assert out.dim() == 3 and out.is_contiguous() and desc.shape == (out.shape[0], 2)
+        mode = {torch.uint8: U8, torch.float32: F32}[out.dtype]
+        n, oh, ow = out.shape
+        self._check(self.lib.b200seg_resize_linear_u8(src.data_ptr(), desc.data_ptr(), n, oh, ow, out.data_ptr(), mode,
+                                                      dev, st))
 
     def mask_logits(self, logits, threshold, mask):
         dev, st = self._ds(logits)

@@ -174,6 +174,8 @@ int normalize_volume(int mode, const float* x, long long nvox, void* ws, long lo
                      cudaStream_t st);
 int resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* ratio, int vD, int vH, int vW, int oD,
                         int oH, int oW, uint8_t* out, int device, cudaStream_t st);
+int resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
+                     int out_mode, cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -913,6 +915,17 @@ int b200seg_resample_nearest_u8(const uint8_t* src, int D, int H, int W, const d
   B200_CHECK_ARG(valid_ratio(ratio_zyx), "b200seg_resample_nearest_u8: ratios must be finite and > 0");
   B200_DEVICE(device);
   return resample_nearest_u8(src, D, H, W, ratio_zyx, vD, vH, vW, oD, oH, oW, out, device, ST(stream));
+}
+
+int b200seg_resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
+                             int out_mode, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(src && desc && out, "b200seg_resize_linear_u8: null argument");
+  B200_CHECK_ARG(n >= 1 && n <= 65535 && oH >= 1 && oW >= 1 && oH <= 65535 * 8,
+                 "b200seg_resize_linear_u8: bad sizes (n %d, %d x %d)", n, oH, oW);
+  B200_CHECK_ARG(out_mode == B200SEG_U8 || out_mode == B200SEG_F32, "b200seg_resize_linear_u8: bad out_mode %d",
+                 out_mode);
+  B200_DEVICE(device);
+  return resize_linear_u8(src, desc, n, oH, oW, out, out_mode, ST(stream));
 }
 
 }  // extern "C"

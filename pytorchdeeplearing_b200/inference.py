@@ -2,7 +2,8 @@
 (model/modelVNet.py:655-676, model/modelUnet.py:641-662), the sliding-window ``inference_patch``
 (model/modelUnet.py:707-763) on the drop-in networks, and the whole-volume 3-D ``XModel.inference`` /
 ``inference_patch`` chains with their SimpleITK resamples and intensity normalisations on the device
-(``inference3d``, ``inference_patch3d``, ``resample3d``; csrc/resample.cu).
+(``inference3d``, ``inference_patch3d``, ``resample3d``; csrc/resample.cu), and the 2-D ``XModel.inference`` with its
+bit-exact cv2 bilinear resizes (``inference2d``, ``resize2d``; csrc/resize2d.cu).
 
 The reference runs the net, copies the fp32 probabilities to the host and thresholds / arg-maxes them with numpy.
 Here the head kernel writes the uint8 mask directly (``b200seg_head_mask``: neither logits nor probs are
@@ -16,7 +17,7 @@ import numpy as np
 import torch
 
 from . import runtime
-from ._abi import NORM_MEANSTD, NORM_NONE, NORM_PCTL
+from ._abi import NORM_MEANSTD, NORM_NONE, NORM_PCTL, resize_src_table
 from .engine import Engine
 
 
@@ -331,5 +332,106 @@ def resample3d(volume, newSize=None, spacing=None, newSpacing=None, interpolator
     return out.cpu().numpy() if is_np else out
 
 
+# ---------------------------------------------------------------------------------------- 2-D image resize and inference
+MAX_RESIZE_BATCH = 65535
+
+
+def resize_desc(be, entries, device) -> torch.Tensor:
+    """[(byte offset, h, w)] of a ragged uint8 batch -> the int64 [N, 2] device table of ``b200seg_resize_src``
+    (uploaded through kernel arguments: no copy from pageable memory, no host synchronisation)"""
+    if not 1 <= len(entries) <= MAX_RESIZE_BATCH:
+        raise ValueError(f"a resize batch holds 1 to {MAX_RESIZE_BATCH} images, got {len(entries)}")
+    raw = resize_src_table(entries)
+    return be.upload_bytes(raw, device)[:len(raw)].view(torch.int64).view(len(entries), 2)
+
+
+def _dsize(dsize):
+    d = tuple(int(v) for v in dsize)
+    if len(d) != 2 or min(d) < 1:
+        raise ValueError(f"dsize must be (width, height) >= 1, got {tuple(dsize)}")
+    return d
+
+
+def resize2d(image, dsize, device="cuda"):
+    """``cv2.resize(image, dsize)`` with its default INTER_LINEAR, bit for bit (csrc/resize2d.cu).  ``dsize`` is
+    (width, height), as in cv2.  ``image``: uint8 (H, W) or a batch (N, H, W), as a numpy array (-> numpy, computed on
+    ``device``) or a tensor (-> a tensor on the tensor's device).  Returns uint8 (height, width) or (N, height, width)."""
+    is_np = not isinstance(image, torch.Tensor)
+    img = torch.from_numpy(np.ascontiguousarray(image)) if is_np else image
+    if img.dtype != torch.uint8:
+        raise TypeError(f"resize2d takes uint8 images, got {img.dtype}")
+    if img.dim() not in (2, 3):
+        raise ValueError(f"expected an (H, W) image or an (N, H, W) batch, got shape {tuple(img.shape)}")
+    if min(img.shape) < 1:
+        raise ValueError(f"image sizes must be >= 1, got {tuple(img.shape)}")
+    ow, oh = _dsize(dsize)
+    batch = img if img.dim() == 3 else img.unsqueeze(0)
+    if is_np:
+        batch = batch.to(device)
+    batch = batch.contiguous()
+    n, h, w = batch.shape
+    be = runtime.get_backend(batch)
+    out = torch.empty((n, oh, ow), dtype=torch.uint8, device=batch.device)
+    be.resize_linear(batch.view(-1), resize_desc(be, [(i * h * w, h, w) for i in range(n)], batch.device), out)
+    if img.dim() == 2:
+        out = out[0]
+    return out.cpu().numpy() if is_np else out
+
+
+@torch.no_grad()
+def _inference2d_device(model, src: torch.Tensor, newSize, out_threshold) -> torch.Tensor:
+    """device uint8 image (h, w) -> device uint8 mask (w, h), or the uint8 class value (1,) of a classifier; no host
+    synchronisation"""
+    be = runtime.get_backend(src)
+    dev = src.device
+    h, w = src.shape
+    W, H = _dsize(newSize)
+    x = torch.empty((1, H, W), dtype=torch.float32, device=dev)
+    be.resize_linear(src.reshape(-1), resize_desc(be, [(0, h, w)], dev), x)       # cv2.resize, then / 255.
+    x = x.view(1, 1, H, W)
+    was_training = model.training
+    model.eval()
+    try:
+        if getattr(model, "_arch", None) == "resnet":
+            logits = model(x).contiguous()                  # (1, numclass) fp32
+            cls = torch.empty((1,), dtype=torch.uint8, device=dev)
+            be.mask_logits(logits, float(out_threshold), cls)
+            return cls
+        m = predict_mask(model, x, out_threshold)[0].contiguous()
+    finally:
+        model.train(was_training)
+    # cv2.resize(out_mask, image.shape): image.shape = (h, w) is read as (width, height)
+    out = torch.empty((1, w, h), dtype=torch.uint8, device=dev)
+    be.resize_linear(m.view(-1), resize_desc(be, [(0, H, W)], dev), out)
+    return out[0]
+
+
+def inference2d(model, image, newSize=(512, 512), out_threshold: float = 0.5):
+    """``XModel.inference(image)`` of a 2-D network (model/modelVNet.py:231-242,450-461, model/modelUnet.py:231-242,
+    450-461, model/modelResNet.py:212-221,428-437): ``cv2.resize(image, newSize)``, ``/ 255.``, ``predict``, and for a
+    segmentation net ``cv2.resize(out_mask, image.shape)``.  ``image``: uint8 (H, W), the output of
+    ``cv2.imread(path, 0)``; ``newSize``: the wrapper's (image_width, image_height).  Only the raw bytes go to the
+    device and only the result comes back; both resizes are bit-exact cv2 INTER_LINEAR.
+
+    Segmentation nets (VNet2d, UNet2d) return a uint8 numpy mask with the reference's two quirks kept: the mask is
+    resized bilinearly (a 0/255 mask gains intermediate values at its edges, class indices are interpolated), and
+    ``dsize = image.shape`` is (height, width) read as (width, height), so an (H, W) image gives a (W, H) mask.
+    ResNet2d returns what the classifier's ``predict`` returns: a numpy int64, 0 / 255 for one class
+    (sigmoid > out_threshold), the arg-max class index otherwise.  3-D networks raise ``ValueError``."""
+    if getattr(model, "_dims", None) != 2:
+        raise ValueError(f"{type(model).__name__} is a 3-D network; inference2d runs the 2-D networks")
+    _dsize(newSize)
+    arr = np.ascontiguousarray(image)
+    if arr.dtype != np.uint8:
+        raise TypeError(f"inference2d takes the uint8 image of cv2.imread(path, 0), got {arr.dtype}")
+    if arr.ndim != 2 or min(arr.shape) < 1:
+        raise ValueError(f"expected an (H, W) image with sizes >= 1, got shape {arr.shape}")
+    dev = next(model.parameters()).device
+    out = _inference2d_device(model, torch.from_numpy(arr).to(dev), newSize, out_threshold)
+    if getattr(model, "_arch", None) == "resnet":
+        return np.int64(out.cpu().numpy()[0])
+    return out.cpu().numpy()
+
+
 __all__ = ["predict_mask", "predict", "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d",
-           "spacing_size"]
+           "spacing_size", "resize2d", "inference2d"]
