@@ -523,6 +523,45 @@ typedef struct b200seg_resize_src {
 int b200seg_resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
                              int out_mode, int device, b200seg_stream stream);
 
+/* ---- 3-D augmentation warp: ImageDataGenerator3D.random_transform + standardize
+ * (dataprocess/Augmentation/images_masks_3dtransform.py, driven by DataAug3D, ImageAugmentation.py:26-75), i.e.
+ * scipy.ndimage.affine_transform(v, M, off, order=0, mode, cval) of every channel and of the label, then the channel
+ * shift, the flips and "x *= rescale".  Per output voxel (d, h, w) of sample s: the flipped axes are un-flipped
+ * (i_a = len_a - 1 - i_a where bit a of param.flip is set); per input axis a of length n,
+ * cc = off[a]; cc += m[3a] i0; cc += m[3a + 1] i1; cc += m[3a + 2] i2 (fp64, each product and sum rounded on its own,
+ * no FMA); cc outside [0, n - 1] is mapped by the mode (NEAREST clamps, CONSTANT fills the whole voxel with cval,
+ * REFLECT / MIRROR / WRAP fold it as scipy's map_coordinate: periods 2n, 2n - 2, n - 1); k = floor(cc + 0.5), an index
+ * one past the edge folded back (REFLECT repeats the edge voxel, MIRROR reflects about it).  The gathered image value
+ * (fp32 cval outside) goes through, in this order: with shift != 0, clip(v + shift[c], min, max) in fp32, min / max
+ * over every channel of the warped sample (numpy's clip: NaN propagates); B200SEG_RESCALE_F32: v * (float)rescale;
+ * B200SEG_RESCALE_F64: (float)((double)v * rescale).  The label (scipy's cval cast outside: fp32 cval, or for uint8
+ * (cval > 0 ? cval + 0.5 : 0) saturated at 255 and truncated) is written as y_dtype, or as int64 (label_out ==
+ * B200SEG_I64: uint8 widened, fp32 truncated toward zero), or with binarize as int64 (y != 0) (model/modelVNet.py:576).
+ * x, x_out: dense [n][D][H][W][C] fp32, C in {1, 3, 4}; y, y_out: dense [n][D][H][W]; y_dtype B200SEG_U8 or
+ * B200SEG_F32; params: device memory, n entries.  With shift a first pass writes per-block min / max partials into ws
+ * (b200seg_augment3d_workspace bytes); min and max do not depend on order, so reruns are bit-identical.
+ * D * H * W < 2^31, n <= 65535; x_out must not alias x. */
+#define B200SEG_AUG_NEAREST 0
+#define B200SEG_AUG_CONSTANT 1
+#define B200SEG_AUG_REFLECT 2
+#define B200SEG_AUG_WRAP 3
+#define B200SEG_AUG_MIRROR 4
+#define B200SEG_RESCALE_NONE 0
+#define B200SEG_RESCALE_F32 1 /* rescale was a Python number: numpy multiplies in fp32 by (float)rescale */
+#define B200SEG_RESCALE_F64 2 /* rescale was a numpy float64: fp64 multiply, rounded once to fp32 */
+typedef struct b200seg_aug3d_param {
+  double m[9];    /* the centred matrix's 3x3 block, row-major */
+  double off[3];  /* its last column */
+  float shift[4]; /* (float) of the channel-shift draw u_c, read when shift != 0 */
+  int32_t flip;   /* bit a set: flip array axis a (0: vertical_flip, 1: horizontal_flip, 2: depth_flip) */
+  int32_t pad;
+} b200seg_aug3d_param; /* 120 bytes */
+int64_t b200seg_augment3d_workspace(int n, int D, int H, int W);
+int b200seg_augment3d(const float* x, const void* y, int y_dtype, int n, int D, int H, int W, int C,
+                      const b200seg_aug3d_param* params, int fill_mode, double cval, int shift, double rescale,
+                      int rescale_mode, float* x_out, void* y_out, int label_out, int binarize, void* ws,
+                      int64_t ws_bytes, int device, b200seg_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,7 +6,9 @@ Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-So
 ``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``), and the whole-volume 3-D inference of
 ``XModel.inference`` / ``inference_patch`` with its resamples and normalisations (``inference3d``,
 ``inference_patch3d``), and the 2-D ``XModel.inference`` and datasets' bit-exact cv2 bilinear resize (``inference2d``,
-``resize2d``, ``InputStager(max_source_pixels=...)``).
+``resize2d``, ``InputStager(max_source_pixels=...)``), and the 3-D data augmentation of
+``dataprocess/Augmentation`` (``ImageDataGenerator3D``: scipy's order-0 affine warp bit for bit, offline through
+``DataAug3D`` or per training step through ``transform_batch``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -28,11 +30,12 @@ from .inference import (predict, predict_mask, sliding_window_mask, inference3d,
                         spacing_size, resize2d, inference2d)
 from .staging import InputStager, stage_batch
 from .ssim import SSIM, SSIM3D, ssim, ssim3D
+from .augment import ImageDataGenerator3D
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
            "predict_mask",
-           "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d", "spacing_size", "resize2d", "inference2d", "InputStager", "stage_batch", "set_precision", "get_precision",
+           "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d", "spacing_size", "resize2d", "inference2d", "ImageDataGenerator3D", "InputStager", "stage_batch", "set_precision", "get_precision",
            "enable_data_parallel", "disable_data_parallel", "install", "uninstall", "GraphedStep",
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",

@@ -136,6 +136,9 @@ _SIGNATURES = {
     "b200seg_normalize": ([_i, _vp, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_resample_nearest_u8": ([_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_resize_linear_u8": ([_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp], C.c_int),
+    "b200seg_augment3d_workspace": ([_i, _i, _i, _i], C.c_int64),
+    "b200seg_augment3d": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, C.c_double, _i, C.c_double, _i, _vp, _vp, _i, _i,
+                           _vp, _i64, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -174,6 +177,22 @@ RESIZE_SRC_BYTES = 16      # sizeof(struct b200seg_resize_src)
 def resize_src_table(entries) -> bytes:
     """[(byte offset, h, w)] of a ragged uint8 batch -> the host bytes of its ``b200seg_resize_src`` table"""
     return b"".join(struct.pack("<qii", int(o), int(h), int(w)) for o, h, w in entries)
+
+
+# fill modes and rescale forms of b200seg_augment3d (B200SEG_AUG_*, B200SEG_RESCALE_*)
+AUG_MODES = {"nearest": 0, "constant": 1, "reflect": 2, "wrap": 3, "mirror": 4}
+RESCALE_NONE, RESCALE_F32, RESCALE_F64 = 0, 1, 2
+AUG3D_PARAM_BYTES = 120    # sizeof(struct b200seg_aug3d_param)
+
+
+def aug3d_param_table(entries) -> bytes:
+    """[(3x3 matrix, offset[3], channel shifts (<= 4 floats), flip bits)] -> the host bytes of a
+    ``b200seg_aug3d_param`` table (fp64 matrix and offset, fp32 shifts, int32 flip bits)"""
+    out = []
+    for m, off, shifts, flip in entries:
+        sh = [float(v) for v in shifts] + [0.0] * (4 - len(shifts))
+        out.append(struct.pack("<9d3d4fii", *[float(v) for v in m], *[float(v) for v in off], *sh, int(flip), 0))
+    return b"".join(out)
 
 
 def _dt(t: torch.Tensor) -> int:
@@ -964,6 +983,30 @@ class CudaBackend:
         n, oh, ow = out.shape
         self._check(self.lib.b200seg_resize_linear_u8(src.data_ptr(), desc.data_ptr(), n, oh, ow, out.data_ptr(), mode,
                                                       dev, st))
+
+    # ------------------------------------------------------------------ 3-D augmentation warp (csrc/augment3d.cu)
+    def augment3d_workspace(self, n, dhw, device):
+        """uint8 workspace of b200seg_augment3d_workspace bytes (the channel shift's min / max partials)"""
+        nb = int(self.lib.b200seg_augment3d_workspace(n, *dhw))
+        return torch.empty(max(nb, 16), dtype=torch.uint8, device=device)
+
+    def augment3d(self, x, y, params, x_out, y_out, mode=0, cval=0.0, shift=False, rescale=0.0,
+                  rescale_mode=RESCALE_NONE, binarize=False, ws=None):
+        """ImageDataGenerator3D's order-0 warp of a batch: x dense fp32 (N, D, H, W, C), C in {1, 3, 4}; y dense
+        uint8 / fp32 (N, D, H, W); params uint8 device bytes of ``aug3d_param_table`` (N entries); x_out like x;
+        y_out like y, or int64 (with ``binarize``: y != 0)"""
+        dev, st = self._ds(x)
+        assert x.dtype == torch.float32 and x.dim() == 5 and x.is_contiguous() and x_out.is_contiguous()
+        assert x_out.dtype == torch.float32 and x_out.shape == x.shape
+        assert y.is_contiguous() and y_out.is_contiguous() and y.shape == x.shape[:4] and y_out.shape == y.shape
+        assert params.dtype == torch.uint8 and params.numel() >= x.shape[0] * AUG3D_PARAM_BYTES
+        codes = {torch.uint8: U8, torch.float32: F32, torch.int64: I64}
+        n, d, h, w, c = x.shape
+        self._check(self.lib.b200seg_augment3d(x.data_ptr(), y.data_ptr(), codes[y.dtype], n, d, h, w, c,
+                                               params.data_ptr(), mode, float(cval), 1 if shift else 0, float(rescale),
+                                               rescale_mode, x_out.data_ptr(), y_out.data_ptr(), codes[y_out.dtype],
+                                               1 if binarize else 0, _p(ws), 0 if ws is None else ws.numel(), dev,
+                                               st))
 
     def mask_logits(self, logits, threshold, mask):
         dev, st = self._ds(logits)

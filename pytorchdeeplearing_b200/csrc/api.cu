@@ -176,6 +176,10 @@ int resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* r
                         int oH, int oW, uint8_t* out, int device, cudaStream_t st);
 int resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
                      int out_mode, cudaStream_t st);
+long long augment3d_workspace(int n, long long vox);
+int augment3d(const float* x, const void* y, int y_dtype, int n, int D, int H, int W, int C,
+              const b200seg_aug3d_param* params, int mode, double cval, int shift, double rescale, int rescale_mode,
+              float* x_out, void* y_out, int label_out, int binarize, void* ws, cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -926,6 +930,38 @@ int b200seg_resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc,
                  out_mode);
   B200_DEVICE(device);
   return resize_linear_u8(src, desc, n, oH, oW, out, out_mode, ST(stream));
+}
+
+static bool valid_aug3d_sizes(int n, int D, int H, int W) {
+  return n >= 1 && n <= 65535 && D >= 1 && H >= 1 && W >= 1 && (long long)D * H * W < (1LL << 31);
+}
+
+int64_t b200seg_augment3d_workspace(int n, int D, int H, int W) {
+  if (!valid_aug3d_sizes(n, D, H, W)) return 0;
+  return augment3d_workspace(n, (long long)D * H * W);
+}
+
+int b200seg_augment3d(const float* x, const void* y, int y_dtype, int n, int D, int H, int W, int C,
+                      const b200seg_aug3d_param* params, int fill_mode, double cval, int shift, double rescale,
+                      int rescale_mode, float* x_out, void* y_out, int label_out, int binarize, void* ws,
+                      int64_t ws_bytes, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(x && y && params && x_out && y_out, "b200seg_augment3d: null argument");
+  B200_CHECK_ARG((const void*)x != (const void*)x_out && y != y_out, "b200seg_augment3d: outputs alias inputs");
+  B200_CHECK_ARG(valid_aug3d_sizes(n, D, H, W),
+                 "b200seg_augment3d: bad sizes (n %d, %d x %d x %d; n <= 65535, D * H * W < 2^31)", n, D, H, W);
+  B200_CHECK_ARG(C == 1 || C == 3 || C == 4, "b200seg_augment3d: C must be 1, 3 or 4 (got %d)", C);
+  B200_CHECK_ARG(y_dtype == B200SEG_U8 || y_dtype == B200SEG_F32, "b200seg_augment3d: bad label dtype %d", y_dtype);
+  B200_CHECK_ARG(label_out == y_dtype || label_out == B200SEG_I64, "b200seg_augment3d: bad label_out %d", label_out);
+  B200_CHECK_ARG(!binarize || label_out == B200SEG_I64, "b200seg_augment3d: binarize writes int64 labels");
+  B200_CHECK_ARG(fill_mode >= B200SEG_AUG_NEAREST && fill_mode <= B200SEG_AUG_MIRROR,
+                 "b200seg_augment3d: bad fill_mode %d", fill_mode);
+  B200_CHECK_ARG(rescale_mode >= B200SEG_RESCALE_NONE && rescale_mode <= B200SEG_RESCALE_F64,
+                 "b200seg_augment3d: bad rescale_mode %d", rescale_mode);
+  B200_CHECK_ARG(!shift || (ws && ws_bytes >= b200seg_augment3d_workspace(n, D, H, W)),
+                 "b200seg_augment3d: the channel shift needs b200seg_augment3d_workspace bytes of workspace");
+  B200_DEVICE(device);
+  return augment3d(x, y, y_dtype, n, D, H, W, C, params, fill_mode, cval, shift, rescale, rescale_mode, x_out, y_out,
+                   label_out, binarize, ws, ST(stream));
 }
 
 }  // extern "C"

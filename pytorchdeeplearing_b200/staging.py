@@ -8,8 +8,9 @@ normalised / widened by two small kernels (csrc/staging.cu), on a side stream, o
 them.  With ``max_source_pixels`` the datasets' ``cv2.resize`` (dataset.py:63,140,154) runs on the device too: the
 images (and labels) of a batch may have any sizes, they are packed into one pinned ragged buffer, sent with one copy,
 resized bit for bit as cv2's INTER_LINEAR (csrc/resize2d.cu) and then staged by the same two kernels.  File reading and
-``cv2.imread`` stay on the host; the 3-D dataset (``datasetModelSegwithnpy``, dataset.py:82-117) stores
-already-normalised float volumes and needs no arithmetic.
+``cv2.imread`` stay on the host; the 3-D dataset (``datasetModelSegwithnpy``, dataset.py:82-117) loads volumes that
+``DataAug3D`` augmented offline and needs no arithmetic itself; that augmentation runs on the device through
+``ImageDataGenerator3D`` (augment.py), offline or per step with ``transform_batch``.
 
     stager = InputStager(device, (8, 512, 512))
     stager.put(images_u8, labels_u8)           # host uint8 arrays/tensors [N, H, W]; returns immediately
