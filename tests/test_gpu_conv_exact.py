@@ -320,13 +320,14 @@ def check_stats(got, v, chain, what):
 
 
 class Guarded:
-    """an (N, D, H, W, C) view with channel pitch ld = C + 16 (C at offset 8 in each row; ld = C with dense=True) in
-    the middle of one allocation with GUARD elements before and after.  Everything outside the view holds `fill`
-    (a float) or the NaN bit pattern of the dtype (fill=None)."""
+    """an (N, D, H, W, C) view with channel pitch ld = C + 16 (C at offset `off` <= 16 in each row, 8 by default;
+    ld = C with dense=True) in the middle of one allocation with GUARD elements before and after.  Everything outside
+    the view holds `fill` (a float) or the NaN bit pattern of the dtype (fill=None)."""
 
-    def __init__(self, shape, dtype, fill=None, device="cpu", dense=False):
+    def __init__(self, shape, dtype, fill=None, device="cpu", dense=False, off=8):
         n, d, h, w, c = shape
-        self.ld, self.off = (c, 0) if dense else (c + 16, 8)
+        assert 0 <= off <= 16
+        self.ld, self.off = (c, 0) if dense else (c + 16, off)
         rows = n * d * h * w
         self.dtype = dtype
         buf = torch.empty(2 * GUARD + rows * self.ld, dtype=dtype)
