@@ -423,9 +423,12 @@ int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const
  * decoupled = 1; torch.optim.Adam model/modelUnet.py:849, decoupled = 0): ONE launch for all parameters instead of
  * ~6 foreach launches over 128 tensors.  state (fp32 [4], device): [0] step count t, [1] lr/(1-b1^t), [2]
  * sqrt(1-b2^t); tick != 0 advances t first (one extra 1-thread launch) so a captured step replays correctly.
- * gscale: optional device scalar multiplied into the gradient (e.g. 1/world for an averaged all-reduce) or NULL. */
+ * gscale: optional device scalar multiplied into the gradient (e.g. 1/world for an averaged all-reduce) or NULL.
+ * lr, the betas and weight_decay are the Python (double) values: as in torch.optim, 1 - beta1, 1 - beta2,
+ * 1 - lr*weight_decay, beta^t and lr/(1-beta1^t) are computed in double and rounded to fp32 once; beta2,
+ * weight_decay and eps enter the elementwise update as their fp32 roundings. */
 int b200seg_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float* state,
-                      float lr, float beta1, float beta2, float eps, float weight_decay, int decoupled,
+                      double lr, double beta1, double beta2, float eps, double weight_decay, int decoupled,
                       const float* gscale, int tick, int device, b200seg_stream stream);
 
 /* ---- ALL dropout channel masks of one forward in one launch (nn.Dropout3d/2d(p), VNet3d.py:11,31,51,67;

@@ -52,7 +52,7 @@ class GnDesc(C.Structure):     # include/b200seg.h: struct b200seg_gn
 
 _PT = C.POINTER(TensorDesc)
 _PG = C.POINTER(GnDesc)
-_vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
+_vp, _i, _i64, _f, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 
 _SIGNATURES = {
     "b200seg_version": ([], C.c_int),
@@ -122,7 +122,7 @@ _SIGNATURES = {
                          C.c_int),
     "b200seg_metric_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _vp, _i, _vp], C.c_int),
     "b200seg_metric_finalize": ([_vp, _i, _i, _vp, _i, _vp], C.c_int),
-    "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _vp, _i, _i, _vp], C.c_int),
+    "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _d, _d, _d, _f, _d, _i, _vp, _i, _i, _vp], C.c_int),
     "b200seg_dropout_masks": ([_vp, _vp, _i, _i, C.c_double, _vp, _i, _vp], C.c_int),
     "b200seg_head_mask": ([_PT, _vp, _vp, _vp, _i, _f, _i, _vp], C.c_int),
     "b200seg_mask_logits": ([_vp, _i64, _i, _f, _vp, _i, _vp], C.c_int),

@@ -115,8 +115,8 @@ int loss_partials(const float* logits, const void* labels, int label_dtype, int 
 int metric_partials(const float* probs, const void* labels, int label_dtype, int N, long long vox, int C, float thr,
                     double* metric, int device, cudaStream_t s);
 int metric_finalize(const double* metric, int N, int C, float* out, cudaStream_t s);
-int adam_step(float* p, const float* g, float* m, float* v, long long n, float* state, float lr, float beta1,
-              float beta2, float eps, float wd, int decoupled, const float* gscale, int tick, int device,
+int adam_step(float* p, const float* g, float* m, float* v, long long n, float* state, double lr, double beta1,
+              double beta2, float eps, double wd, int decoupled, const float* gscale, int tick, int device,
               cudaStream_t s);
 int dropout_masks(const long long* rng, const int* table, int nmasks, int total, double p_drop, float* out,
                   cudaStream_t s);
@@ -661,7 +661,7 @@ int b200seg_metric_finalize(const double* metric, int N, int C, float* out, int 
 }
 
 int b200seg_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float* state,
-                      float lr, float beta1, float beta2, float eps, float weight_decay, int decoupled,
+                      double lr, double beta1, double beta2, float eps, double weight_decay, int decoupled,
                       const float* gscale, int tick, int device, b200seg_stream stream) {
   B200_CHECK_ARG(param && grad && exp_avg && exp_avg_sq && state && n > 0, "b200seg_adam_step: bad argument");
   B200_DEVICE(device);

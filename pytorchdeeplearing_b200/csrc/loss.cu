@@ -338,11 +338,12 @@ __global__ void loss_finalize_kernel(const double* __restrict__ part, int C, int
 }
 
 // d/dce of (1-pt)^gamma * ce with pt = exp(-ce):  (1-pt)^gamma + gamma (1-pt)^(gamma-1) pt ce
+// At om = 0 the limit is 1 for gamma = 0 ((1-pt)^0 = 1), pt ce for gamma = 1 and 0 for every other gamma > 0.
 __device__ __forceinline__ float focal_factor(float ce, float gamma) {
   const float pt = expf(-ce);
   const float om = 1.f - pt;
   if (gamma == 2.f) return om * om + 2.f * om * pt * ce;
-  if (om <= 0.f) return gamma == 1.f ? pt * ce : 0.f;
+  if (om <= 0.f) return gamma == 0.f ? 1.f : (gamma == 1.f ? pt * ce : 0.f);
   return powf(om, gamma) + gamma * powf(om, gamma - 1.f) * pt * ce;
 }
 

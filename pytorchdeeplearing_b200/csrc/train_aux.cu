@@ -19,28 +19,29 @@ namespace b200seg {
 //   p -= (lr / (1 - b1^t)) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
 // state[0] = t (step count, fp32 like torch's step tensor), state[1] = lr / (1 - b1^t), state[2] = sqrt(1 - b2^t)
 // The step count lives on the device so that the update can be replayed from a CUDA graph.
+// Like torch, every constant (1 - b1, 1 - b2, 1 - lr wd, b^t, lr / bc1) is computed in double from the double
+// hyper-parameters and rounded to fp32 once: 1.f - 0.999f is 111 fp32 ulps away from (float)(1 - 0.999).
 // ------------------------------------------------------------------------------------------------
-__global__ void adam_tick_kernel(float* __restrict__ state, float lr, float beta1, float beta2) {
+__global__ void adam_tick_kernel(float* __restrict__ state, double lr, double beta1, double beta2) {
   PDL_ENTER();
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
   const double t = (double)state[0] + 1.0;
   state[0] = (float)t;
-  const double bc1 = 1.0 - pow((double)beta1, t);
-  const double bc2 = 1.0 - pow((double)beta2, t);
-  state[1] = (float)((double)lr / bc1);
+  const double bc1 = 1.0 - pow(beta1, t);
+  const double bc2 = 1.0 - pow(beta2, t);
+  state[1] = (float)(lr / bc1);
   state[2] = (float)sqrt(bc2);
 }
 
+// w1 = 1 - b1, w2 = 1 - b2, decay = 1 - lr wd: each the fp32 rounding of the double value
 __global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ p, const float* __restrict__ g,
                                                         float* __restrict__ m, float* __restrict__ v, long long n,
-                                                        const float* __restrict__ state, float lr, float beta1,
-                                                        float beta2, float eps, float wd, int decoupled,
+                                                        const float* __restrict__ state, float w1, float w2,
+                                                        float beta2, float eps, float wd, float decay, int decoupled,
                                                         const float* __restrict__ gscale, long long n4) {
   PDL_ENTER();
   const float step_size = state[1], bc2s = state[2];
   const float gs = gscale ? gscale[0] : 1.f;
-  const float decay = 1.f - lr * wd;
-  const float w1 = 1.f - beta1, w2 = 1.f - beta2;
   const long long stride = (long long)gridDim.x * blockDim.x;      // n4: float4 groups (0 when a buffer is unaligned)
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
     float4 pv = reinterpret_cast<float4*>(p)[i];
@@ -74,8 +75,8 @@ __global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ p, c
   }
 }
 
-int adam_step(float* p, const float* g, float* m, float* v, long long n, float* state, float lr, float beta1,
-              float beta2, float eps, float wd, int decoupled, const float* gscale, int tick, int device,
+int adam_step(float* p, const float* g, float* m, float* v, long long n, float* state, double lr, double beta1,
+              double beta2, float eps, double wd, int decoupled, const float* gscale, int tick, int device,
               cudaStream_t s) {
   const bool al = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                     reinterpret_cast<uintptr_t>(v)) % 16) == 0;
@@ -85,8 +86,8 @@ int adam_step(float* p, const float* g, float* m, float* v, long long n, float* 
   const long long cap = (long long)num_sms(device) * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  launch_k(adam_step_kernel, (int)blocks, 256, 0, s, p, g, m, v, n, state, lr, beta1, beta2, eps, wd, decoupled, gscale,
-                                               n4);
+  launch_k(adam_step_kernel, (int)blocks, 256, 0, s, p, g, m, v, n, state, (float)(1.0 - beta1),
+           (float)(1.0 - beta2), (float)beta2, eps, (float)wd, (float)(1.0 - lr * wd), decoupled, gscale, n4);
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
 }
