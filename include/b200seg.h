@@ -294,6 +294,17 @@ int b200seg_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dim
 int b200seg_pool_bwd(const b200seg_tensor* x, const b200seg_tensor* g_out, const b200seg_tensor* addend,
                      const b200seg_tensor* g_x, int dims, int device, b200seg_stream stream);
 
+/* ---- UNet3dthin's decoder join (Unet3dthin.py:40-54): nn.Upsample(scale_factor=2, mode='trilinear') + torch.add.
+ * S (N, 2d, 2h, 2w, C) = up2(a) + e for a (N, d, h, w, C); e has S's shape.  up2 is torch's upsample_trilinear3d with
+ * align_corners=False: per axis fine 2k reads coarse (k-1, k) with (1/4, 3/4), fine 2k+1 reads (k, k+1) with (3/4, 1/4),
+ * and the edges clamp (fine 0 and fine 2n-1 take coarse 0 and n-1 with weight 1).  Sums in fp32, one rounding to the
+ * storage type.  The backward writes ga = up2^T(gS), a fixed-order gather (no atomics); the skip's gradient is gS
+ * itself.  All tensors share one dtype (F32 or BF16); C and every pitch are multiples of 8, every pointer 16-byte
+ * aligned; any coarse extent >= 1. */
+int b200seg_upsample2_add(const b200seg_tensor* a, const b200seg_tensor* e, const b200seg_tensor* s, int device,
+                          b200seg_stream stream);
+int b200seg_upsample2_bwd(const b200seg_tensor* g_s, const b200seg_tensor* g_a, int device, b200seg_stream stream);
+
 /* ---- fused head (OutputTransition3d, VNet3d.py:90-99; Unet3d.py:56-61): 1x1 conv to `nc` <= 8 classes + bias,
  * then sigmoid (nc == 1) or softmax over classes.  w: the nn.Conv parameter itself, fp32 [nc][Cin]; logits and
  * probs: fp32 channels-last [voxels][nc]; probs may be NULL (logits only). */

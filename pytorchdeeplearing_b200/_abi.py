@@ -86,6 +86,8 @@ _SIGNATURES = {
     "b200seg_colsum": ([_PT, _vp, _i, _vp], C.c_int),
     "b200seg_pool_fwd": ([_PT, _PT, _i, _i, _vp], C.c_int),
     "b200seg_pool_bwd": ([_PT, _PT, _PT, _PT, _i, _i, _vp], C.c_int),
+    "b200seg_upsample2_add": ([_PT, _PT, _PT, _i, _vp], C.c_int),
+    "b200seg_upsample2_bwd": ([_PT, _PT, _i, _vp], C.c_int),
     "b200seg_head_probs": ([_vp, _vp, _i64, _i, _i, _vp], C.c_int),
     "b200seg_head_fwd": ([_PT, _vp, _vp, _vp, _vp, _i, _i, _vp], C.c_int),
     "b200seg_stem_gn_supported": ([_PT, _i, _i], C.c_int),
@@ -650,6 +652,19 @@ class CudaBackend:
         dev, st = self._ds(x)
         dx, dg, da, do = _desc(x), _desc(g_out), _desc(addend), _desc(g_x)
         self._check(self.lib.b200seg_pool_bwd(C.byref(dx), C.byref(dg), _ref(da), C.byref(do), dims, dev, st))
+
+    # ------------------------------------------------------------------ trilinear 2x upsample + skip add (UNet3dthin)
+    def upsample_add(self, a, e, s):
+        """s (N,2D,2H,2W,C) = up2(a) + e for a (N,D,H,W,C); e has s's shape"""
+        dev, st = self._ds(a)
+        da, de, ds = _desc(a), _desc(e), _desc(s)
+        self._check(self.lib.b200seg_upsample2_add(C.byref(da), C.byref(de), C.byref(ds), dev, st))
+
+    def upsample_bwd(self, g_s, g_a):
+        """g_a (N,D,H,W,C) = up2^T(g_s), written"""
+        dev, st = self._ds(g_s)
+        dg, da = _desc(g_s), _desc(g_a)
+        self._check(self.lib.b200seg_upsample2_bwd(C.byref(dg), C.byref(da), dev, st))
 
     # ------------------------------------------------------------------ head + losses
     def head_probs(self, logits, probs):

@@ -106,6 +106,9 @@ int ew_gn_bwd_apply(const b200seg_tensor* g, const b200seg_tensor* y, const floa
                     const b200seg_gn* gn, const double* sums, float* dgamma, float* dbeta, float* dbias,
                     const b200seg_tensor* dy, int device, cudaStream_t s, int sum_y_from_stats = 0);
 int ew_colsum(const b200seg_tensor* dy, float* out, int device, cudaStream_t s);
+int upsample2_add(const b200seg_tensor* a, const b200seg_tensor* e, const b200seg_tensor* s, int device,
+                  cudaStream_t st);
+int upsample2_bwd(const b200seg_tensor* gs, const b200seg_tensor* ga, int device, cudaStream_t st);
 int ew_pool_fwd(const b200seg_tensor* x, const b200seg_tensor* out, int dims, int device, cudaStream_t s);
 int ew_pool_bwd(const b200seg_tensor* x, const b200seg_tensor* go, const b200seg_tensor* addend,
                 const b200seg_tensor* gx, int dims, int device, cudaStream_t s);
@@ -607,6 +610,22 @@ int b200seg_pool_bwd(const b200seg_tensor* x, const b200seg_tensor* g_out, const
   B200_CHECK_ARG(dims == 2 || dims == 3, "b200seg_pool_bwd: dims must be 2 or 3");
   B200_DEVICE(device);
   return ew_pool_bwd(x, g_out, addend, g_x, dims, device, ST(stream));
+}
+
+int b200seg_upsample2_add(const b200seg_tensor* a, const b200seg_tensor* e, const b200seg_tensor* s, int device,
+                          b200seg_stream stream) {
+  REQ_TENSOR(a, "a");
+  REQ_TENSOR(e, "e");
+  REQ_TENSOR(s, "s");
+  B200_DEVICE(device);
+  return upsample2_add(a, e, s, device, ST(stream));
+}
+
+int b200seg_upsample2_bwd(const b200seg_tensor* g_s, const b200seg_tensor* g_a, int device, b200seg_stream stream) {
+  REQ_TENSOR(g_s, "g_s");
+  REQ_TENSOR(g_a, "g_a");
+  B200_DEVICE(device);
+  return upsample2_bwd(g_s, g_a, device, ST(stream));
 }
 
 int b200seg_head_fwd(const b200seg_tensor* x, const float* w, const float* bias, float* logits, float* probs, int nc,

@@ -75,14 +75,15 @@ OV_ALL = OV_PACK | OV_UNPACK | OV_TAIL | OV_ZERO
 
 def overlap_mask(arch: str = "vnet", dims: int = 3) -> int:
     """``B200SEG_OVERLAP`` if set, else the default: all four options together for VNet3d / VNet2d / UNet2d on one GPU,
-    the plain schedule for the 3-D UNet and for data-parallel runs (``tools/overlap_ab.py`` is the A/B harness)."""
+    the plain schedule for the 3-D UNets (UNet3d, UNet3dthin) and for data-parallel runs (``tools/overlap_ab.py`` is the
+    A/B harness)."""
     e = os.environ.get("B200SEG_OVERLAP")
     if e is not None:
         try:
             return int(e) & OV_ALL
         except ValueError:
             return 0
-    if arch == "unet" and dims == 3:
+    if arch in ("unet", "unetthin") and dims == 3:
         return 0
     from . import runtime
     if runtime.dp_state()[0]:
@@ -947,6 +948,95 @@ class Engine:
             e, pooled = sv[f"pool{i + 1}"]
             ge = torch.empty(e.shape, dtype=self.T, device=e.device)
             self.be.pool_bwd(e, g, genc[i], ge, self.dims)               # + gradient from the skip concat
+            L1, L2 = sv[f"encoder{i + 1}"]
+            g1 = self.bwd_layer(L2, ge, True, prev=L1)
+            g = self.bwd_layer(L1, g1, i > 0)
+        self._finish_backward()
+        return flat
+
+    # ================================================================== UNet3dthin
+    def unetthin_forward(self, P: Dict[str, Tensor], x: Tensor, masks: Optional[List[Tensor]],
+                         need_grad: bool) -> Tuple[Tensor, Tensor]:
+        """UNet3dthin.forward (reference networks/Unet3dthin.py:33-62): UNet3d's encoder, then four decoder blocks at
+        the coarse resolution of their level, each followed by ``S = up2(block output) + encoder output``
+        (nn.Upsample(2, trilinear) + torch.add, one kernel).  3-D only."""
+        self.P, self.masks, self._mi, self.layers, self.need_grad = P, masks, 0, [], need_grad
+        sv = self.saved = {}
+        n, cin = x.shape[0], x.shape[1]
+        self._begin_pass(n, x.device, backward=False)
+        sp0 = tuple(x.shape[2:])
+        xin = x.permute(0, 2, 3, 4, 1)
+        if cin != 1:
+            xin = xin.contiguous()
+        f = P["encoder1.enc1conv1.weight"].shape[0]
+        ch = [f, 2 * f, 4 * f, 8 * f, 16 * f]
+        sps = [sp0]
+        for _ in range(4):
+            s = sps[-1]
+            sps.append((s[0] // 2, s[1] // 2, s[2] // 2))
+        vox = [sp[0] * sp[1] * sp[2] for sp in sps]
+        specs = []
+        for i, (mod, name) in enumerate((("encoder1", "enc1"), ("encoder2", "enc2"), ("encoder3", "enc3"),
+                                         ("encoder4", "enc4"), ("bottleneck", "bottleneck"))):
+            specs.append((f"{mod}.{name}conv1.weight", K3, vox[i], vox[i], i > 0))
+            specs.append((f"{mod}.{name}conv2.weight", K3, vox[i], vox[i], True))
+        for k in (4, 3, 2, 1):                              # decoder k runs at level k (the coarse side of its join)
+            specs.append((f"decoder{k}.dec{k}conv1.weight", K3, vox[k], vox[k], True))
+            specs.append((f"decoder{k}.dec{k}conv2.weight", K3, vox[k], vox[k], True))
+        self._batch, self._ov = n, overlap_mask("unetthin", 3)
+        self._prepack(specs, need_grad, n_early=2)         # encoder1
+
+        def block(mod: str, name: str, h: Tensor, sp, co: int) -> Tensor:
+            L1 = self.conv_gn(K3, f"{mod}.{name}conv1.weight", None, f"{mod}.{name}norm1", h, sp, co)
+            a1 = self.act(L1, self.new(x, sp, co))
+            L2 = self.conv_gn(K3, f"{mod}.{name}conv2.weight", None, f"{mod}.{name}norm2", a1, sp, co)
+            a2 = self.act(L2, self.new(x, sp, co))
+            sv[mod] = (L1, L2)
+            return a2
+
+        h = xin
+        encs = []
+        for i in range(4):
+            e = block(f"encoder{i + 1}", f"enc{i + 1}", h, sps[i], ch[i])
+            encs.append(e)
+            h = self.new(x, sps[i + 1], ch[i])
+            self.be.pool_fwd(e, h, 3)                                      # nn.MaxPool3d(2, 2), Unet3dthin.py:18-24
+            sv[f"pool{i + 1}"] = (e, h)
+        h = block("bottleneck", "bottleneck", h, sps[4], ch[4])
+        for k in (4, 3, 2, 1):
+            d = block(f"decoder{k}", f"dec{k}", h, sps[k], ch[k - 1])
+            self._tag(f"decoder{k}")
+            h = self.new(x, sps[k - 1], ch[k - 1])
+            self.be.upsample_add(d, encs[k - 1], h)                       # Unet3dthin.py:41-42 (47, 51, 54)
+        ncls = P["conv.weight"].shape[0]
+        Lh, logits, probs = self.head("conv.weight", "conv.bias", h, sp0, ncls)
+        sv["head"] = Lh
+        return self._out_views(logits, probs)
+
+    def unetthin_backward(self, g_logits: Tensor) -> Tensor:
+        """Gradients of all 56 parameters given d loss / d logits.  The gradient of each join ``S_k`` goes twice: through
+        up2^T into decoder k, and unchanged into the skip, where it is the addend of encoder k's max-pool backward."""
+        sv = self.saved
+        flat = self.alloc_grads(g_logits.device)
+        self._begin_pass(g_logits.shape[0], g_logits.device, backward=True)
+        g = self.head_backward(sv["head"], g_logits)
+        gS: List[Optional[Tensor]] = [None] * 4
+        for k in (1, 2, 3, 4):
+            gS[k - 1] = g
+            L1, L2 = sv[f"decoder{k}"]
+            self._tag(f"decoder{k}")
+            gd = torch.empty(L2.y.shape, dtype=self.T, device=g.device)
+            self.be.upsample_bwd(g, gd)
+            g1 = self.bwd_layer(L2, gd, True, prev=L1)
+            g = self.bwd_layer(L1, g1, True)
+        L1, L2 = sv["bottleneck"]
+        g = self.bwd_layer(L1, self.bwd_layer(L2, g, True, prev=L1), True)
+        self._flush_bucket("bottleneck.bottleneckconv1.weight")
+        self._early_unpack()
+        for i in (3, 2, 1, 0):
+            e, pooled = sv[f"pool{i + 1}"]
+            ge = torch.empty(e.shape, dtype=self.T, device=e.device)
+            self.be.pool_bwd(e, g, gS[i], ge, 3)                         # + the skip's gradient
             L1, L2 = sv[f"encoder{i + 1}"]
             g1 = self.bwd_layer(L2, ge, True, prev=L1)
             g = self.bwd_layer(L1, g1, i > 0)

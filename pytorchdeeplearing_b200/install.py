@@ -2,7 +2,7 @@
 
 The reference wrappers bind the classes at import time (``from networks.VNet3d import VNet3d``
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
-rebinds those names in whichever of ``networks``, ``networks.*``, ``model.modelVNet``,
+rebinds those names in whichever of ``networks``, ``networks.*`` (``networks.Unet3dthin`` included), ``model.modelVNet``,
 ``model.modelUnet``, ``model.modelResNet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM`` are already imported (and in ``sys.modules`` entries
 imported later via the same names).  ``ImageDataGenerator3D`` is rebound in ``dataprocess.Augmentation.
 images_masks_3dtransform`` and ``dataprocess.Augmentation.ImageAugmentation`` (which binds it at import,
@@ -15,7 +15,7 @@ import sys
 
 _SAVED = []
 
-_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet2d", "ResNet2d", "ResNet3d")
+_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet2d", "ResNet3d")
 _METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "Seg_Metirc3d")
 _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
@@ -24,7 +24,8 @@ _EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "Bin
                    "LovaszLoss")
 # model/lossesSSIM.py
 _SSIM_NAMES = ("SSIM", "SSIM3D", "ssim", "ssim3D")
-_MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet2d", "model",
+_MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet3dthin", "networks.Unet2d",
+            "model",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
             "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet",
             "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation")

@@ -3,6 +3,7 @@ from torch import nn
 
 from .Unet2d import UNet2d
 from .Unet3d import UNet3d
+from .Unet3dthin import UNet3dthin
 from .VNet3d import VNet3d
 from .VNet2d import VNet2d
 from .ResNet2d import ResNet2d
@@ -27,4 +28,4 @@ def initialize_weights(net):
         nn.init.constant_(net.bias.data, 0)
 
 
-__all__ = ["UNet2d", "UNet3d", "VNet3d", "VNet2d", "ResNet2d", "ResNet3d", "initialize_weights"]
+__all__ = ["UNet2d", "UNet3d", "UNet3dthin", "VNet3d", "VNet2d", "ResNet2d", "ResNet3d", "initialize_weights"]

@@ -1,9 +1,29 @@
-"""Shared builder of the drop-in UNet3d / UNet2d (reference networks/Unet3d.py, Unet2d.py)."""
+"""Shared builder of the drop-in UNet3d / UNet2d / UNet3dthin (reference networks/Unet3d.py, Unet2d.py,
+Unet3dthin.py)."""
 from collections import OrderedDict
 
 import torch.nn as nn
 
 from ._base import SegNetBase
+
+
+def unet_block(Conv, ci, co, name):
+    """(conv3 no-bias -> GroupNorm(8) -> Dropout(.2) -> ReLU) x2, Unet3d.py:65-86 (Unet3dthin.py:64-86 is the same
+    block); only the stateful members are registered (dropout / relu carry no state_dict entries)"""
+    return nn.Sequential(OrderedDict([
+        (name + "conv1", Conv(ci, co, kernel_size=3, padding=1, bias=False)),
+        (name + "norm1", nn.GroupNorm(8, co)),
+        (name + "conv2", Conv(co, co, kernel_size=3, padding=1, bias=False)),
+        (name + "norm2", nn.GroupNorm(8, co)),
+    ]))
+
+
+def unet_mask_channels(f):
+    """channels of the 18 dropout calls, in module-call order (two per block: encoders, bottleneck, decoders)"""
+    ch = []
+    for c in (f, 2 * f, 4 * f, 8 * f, 16 * f, 8 * f, 4 * f, 2 * f, f):
+        ch += [c, c]
+    return ch
 
 
 class _UNetBase(SegNetBase):
@@ -18,14 +38,7 @@ class _UNetBase(SegNetBase):
         self.out_channels = out_channels
 
         def block(ci, co, name):
-            # (conv3 no-bias -> GroupNorm(8) -> Dropout(.2) -> ReLU) x2, Unet3d.py:65-86; only the
-            # stateful members are registered (dropout / relu carry no state_dict entries)
-            return nn.Sequential(OrderedDict([
-                (name + "conv1", Conv(ci, co, kernel_size=3, padding=1, bias=False)),
-                (name + "norm1", nn.GroupNorm(8, co)),
-                (name + "conv2", Conv(co, co, kernel_size=3, padding=1, bias=False)),
-                (name + "norm2", nn.GroupNorm(8, co)),
-            ]))
+            return unet_block(Conv, ci, co, name)
 
         self.encoder1 = block(in_channels, f, "enc1")
         self.encoder2 = block(f, 2 * f, "enc2")
@@ -44,8 +57,4 @@ class _UNetBase(SegNetBase):
         self._finish_init()
 
     def _mask_channels(self):
-        f = self.features
-        ch = []
-        for c in (f, 2 * f, 4 * f, 8 * f, 16 * f, 8 * f, 4 * f, 2 * f, f):
-            ch += [c, c]
-        return ch
+        return unet_mask_channels(self.features)

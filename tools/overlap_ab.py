@@ -72,6 +72,12 @@ def main():
     elif args.workload == "unet3d":
         model, ncls, shape = b200.UNet3d(1, 4), 4, (1, 1, 128, 128, 128)
         lossfn = b200.MutilCrossEntropyDiceLoss(torch.ones(4, device=dev))
+    elif args.workload == "unet3dthin":
+        model, ncls, shape = b200.UNet3dthin(1, 2), 2, (2, 1, 96, 96, 96)
+        lossfn = b200.MutilDiceLoss(torch.ones(2, device=dev))
+    elif args.workload == "unet3dthin128":
+        model, ncls, shape = b200.UNet3dthin(1, 5), 5, (1, 1, 128, 112, 112)
+        lossfn = b200.MutilCrossEntropyDiceLoss(torch.ones(5, device=dev))
     else:
         model, ncls, shape = b200.UNet2d(1, 1), 1, (8, 1, 512, 512)
         lossfn = b200.BinaryDiceFocalLoss()
