@@ -194,7 +194,7 @@ def ref_wgrad(ws, a, b):
     """dwp[t][ca][cb] from autograd of the layer conv y = conv(a, W) with dL/dy = b (parameter layout (cb, ca, k))"""
     kind, dims = ws["kind"], ws["dims"]
     k = _k(kind, dims)
-    w0 = torch.zeros((ws["cb"], ws["ca"]) + k, dtype=torch.float64, requires_grad=True)
+    w0 = torch.zeros((ws["cb"], ws["ca"]) + k, dtype=torch.float64, device=a.device, requires_grad=True)
     pad = (k[0] // 2, k[1] // 2, k[2] // 2) if kind == K3 else 0
     stride = k if kind == DOWN else 1
     with torch.enable_grad():
