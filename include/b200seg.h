@@ -430,6 +430,48 @@ int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const
                      int size_average, const float* gout, const double* acc, float* grad1, float* grad2, int device,
                      b200seg_stream stream);
 
+/* ---- soft-clDice (model/lossescldice.py, with its four defects repaired: DESIGN.md section 2).  Shapes are (N, C, D,
+ * H, W) (2-D: pass D = 1).  A field is fp32 with element strides {n, c, d, h, w} (host int64 [5], read during the call;
+ * NCDHW and channels-last views alike), or, where a *_labels pointer is given instead, the one-hot of dense int64
+ * labels [N][D][H][W] (value 1 where label == c).  One skeleton round is, in fp32 and bit-identical to torch:
+ * m = minpool(x), M = maxpool(m), x' = relu(x - relu(M - m)), 3x3x3 pools (3x3 when D = 1), stride 1, padding 1.
+ * b200seg_cldice_skeleton runs `rounds` (1..64) rounds; round r writes fields + (r % nfields) * N*C*D*H*W (dense
+ * NCDHW; nfields >= min(rounds, 2); nfields = rounds keeps every round for the backward).  With `other` (or
+ * other_labels) the last round also writes per-CTA fp64 sums {sum x' * other, sum x'} into half `pass` (0: pred's
+ * skeleton against the target, 1: the target's against pred) of `workspace` (b200seg_cldice_workspace bytes); a labels
+ * pass also counts labels outside [0, C).
+ * b200seg_cldice_finalize: stats fp64 [N*C*8 + 3*G + 1] = per (n, c) {sum sk(p) t, sum sk(p), sum sk(t) p, sum sk(t),
+ * iflat, tflat, d loss / d iflat, d loss / d tflat}, then the G group sums {sum iflat * tflat, sum iflat, sum tflat}
+ * (G = C with per_class, else 1), then the count of bad labels (labels != 0).  loss fp32 [1]: binary
+ * 1 - (2 I + smooth) / max(sum iflat + sum tflat + smooth, eps), or per class with alpha (device fp32 [C]) weights,
+ * summed and divided by C.  reduce == 0 starts from the group sums (after a data-parallel all-reduce of them).
+ * b200seg_cldice_bwd: grad (dense fp32 (N, C, D, H, W)) = d / d x of the `rounds` rounds run on x, from fields
+ * [rounds][N*C*D*H*W] of the skeleton pass (nfields = rounds) and scratch (one dense field; both unused when rounds = 1).
+ * The seed is grad_skeleton (dense fp32), or, when that is NULL, the loss: gout (device fp32 [1]) times d loss / d
+ * sk(pred) from the target and stats, plus the direct tflat term from target_skeleton.  Fixed-order gathers, no atomics.
+ * b200seg_cldice_norm: out fp32 [N*C] = (sum cl * vessel + 1) / (sum cl + 1) and sums fp64 [N*C][2] = {sum cl *
+ * vessel, sum cl}; b200seg_cldice_norm_bwd: grad_cl / grad_vessel (dense fp32, either may be NULL) from gout
+ * (fp32 [N*C]) and sums. */
+int64_t b200seg_cldice_workspace(int N, int C, int D, int H, int W);
+int b200seg_cldice_skeleton(const float* x, const int64_t* x_strides, const int64_t* x_labels, int N, int C, int D,
+                            int H, int W, int rounds, float* fields, int nfields, const float* other,
+                            const int64_t* other_strides, const int64_t* other_labels, int pass, void* workspace,
+                            int64_t workspace_bytes, int device, b200seg_stream stream);
+int b200seg_cldice_finalize(int N, int C, int D, int H, int W, int per_class, int labels, const float* alpha,
+                            double smooth, double eps, int reduce, const void* workspace, int64_t workspace_bytes,
+                            double* stats, float* loss, int device, b200seg_stream stream);
+int b200seg_cldice_bwd(const float* x, const int64_t* x_strides, int N, int C, int D, int H, int W, int rounds,
+                       const float* fields, const float* grad_skeleton, const float* target,
+                       const int64_t* target_strides, const int64_t* target_labels, const float* target_skeleton,
+                       const double* stats, const float* gout, float* grad, float* scratch, int device,
+                       b200seg_stream stream);
+int b200seg_cldice_norm(const float* cl, const int64_t* cl_strides, const float* vessel, const int64_t* vessel_strides,
+                        int N, int C, int D, int H, int W, double* sums, float* out, int device,
+                        b200seg_stream stream);
+int b200seg_cldice_norm_bwd(const float* cl, const int64_t* cl_strides, const float* vessel,
+                            const int64_t* vessel_strides, int N, int C, int D, int H, int W, const double* sums,
+                            const float* gout, float* grad_cl, float* grad_vessel, int device, b200seg_stream stream);
+
 /* ---- fused optimizer step over FLAT fp32 buffers (torch.optim.AdamW(lr) model/modelVNet.py:548, weight_decay 0.01,
  * decoupled = 1; torch.optim.Adam model/modelUnet.py:849, decoupled = 0): ONE launch for all parameters instead of
  * ~6 foreach launches over 128 tensors.  state (fp32 [4], device): [0] step count t, [1] lr/(1-b1^t), [2]

@@ -3,7 +3,9 @@ junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
 ``networks/Unet3dthin.py``, ``networks/Unet2d.py`` forward/backward, the ``networks/ResNet3d.py`` / ``ResNet2d.py`` classifiers and the losses of ``model/losses.py`` (Dice / BCE / focal / CE,
 Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8), and the
 3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``) and the SSIM losses of
-``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``), and the whole-volume 3-D inference of
+``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``), the soft-clDice losses of ``model/lossescldice.py``
+(``soft_skeletonize``, ``norm_intersection``, ``Binary_Soft_cldice_loss``, ``Mutil_Soft_cldice_loss``; the reference
+module raises as shipped, so its evident intent runs here, with four documented repairs), and the whole-volume 3-D inference of
 ``XModel.inference`` / ``inference_patch`` with its resamples and normalisations (``inference3d``,
 ``inference_patch3d``), and the 2-D ``XModel.inference`` and datasets' bit-exact cv2 bilinear resize (``inference2d``,
 ``resize2d``, ``InputStager(max_source_pixels=...)``), and the 3-D data augmentation of
@@ -31,6 +33,7 @@ from .inference import (predict, predict_mask, sliding_window_mask, inference3d,
 from .staging import InputStager, stage_batch
 from .ssim import SSIM, SSIM3D, ssim, ssim3D
 from .augment import ImageDataGenerator3D
+from .cldice import soft_skeletonize, norm_intersection, Binary_Soft_cldice_loss, Mutil_Soft_cldice_loss
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
@@ -40,4 +43,5 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
            "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
-           "MutilELDiceLoss", "LovaszLoss", "SSIM", "SSIM3D", "ssim", "ssim3D"]
+           "MutilELDiceLoss", "LovaszLoss", "SSIM", "SSIM3D", "ssim", "ssim3D",
+           "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss"]

@@ -122,6 +122,14 @@ _SIGNATURES = {
     "b200seg_ssim_finalize": ([_i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i64, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_ssim_bwd": ([_i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp],
                          C.c_int),
+    "b200seg_cldice_workspace": ([_i, _i, _i, _i, _i], C.c_int64),
+    "b200seg_cldice_skeleton": ([_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _i64, _i, _vp],
+                                C.c_int),
+    "b200seg_cldice_finalize": ([_i, _i, _i, _i, _i, _i, _i, _vp, _d, _d, _i, _vp, _i64, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_cldice_bwd": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp],
+                           C.c_int),
+    "b200seg_cldice_norm": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_cldice_norm_bwd": ([_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_metric_partials": ([_vp, _vp, _i, _i, _i64, _i, _f, _vp, _i, _vp], C.c_int),
     "b200seg_metric_finalize": ([_vp, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_adam_step": ([_vp, _vp, _vp, _vp, _i64, _vp, _d, _d, _d, _f, _d, _i, _vp, _i, _i, _vp], C.c_int),
@@ -865,6 +873,70 @@ class CudaBackend:
                                               *geom[1:], window_size, C.cast(t, _vp), coef.data_ptr(),
                                               int(bool(size_average)), gout.data_ptr(), acc.data_ptr(), _p(grad1),
                                               _p(grad2), dev, st))
+
+    # ------------------------------------------------------------------ soft-clDice (model/lossescldice.py)
+    @staticmethod
+    def _cl_field(t):
+        """(float pointer, host strides, labels pointer) of an fp32 (N, C, [D,] H, W) field, or of int64 labels
+        (N, [D,] H, W) whose one-hot stands for the field"""
+        if t is None:
+            return None, None, None
+        if t.dtype == torch.int64:
+            return None, None, t.data_ptr()
+        _, s = CudaBackend._ssim_geom(t)
+        return t.data_ptr(), s, None
+
+    @staticmethod
+    def _cl_shape(x):
+        return (x.shape[0], x.shape[1], 1) + tuple(x.shape[2:]) if x.dim() == 4 else tuple(x.shape)
+
+    def cldice_workspace(self, x):
+        nb = int(self.lib.b200seg_cldice_workspace(*self._cl_shape(x)))
+        return torch.empty(max(nb, 8) // 8, dtype=torch.float64, device=x.device)
+
+    def cldice_skeleton(self, x, rounds, fields, other=None, pass_=0, ws=None):
+        """x fp32 (any strides) or int64 labels with ``fields``' (N, C) leading extents; fields fp32 [nfields][...];
+        other (fp32 or int64 labels) adds the epilogue sums into half ``pass_`` of ``ws``"""
+        dev, st = self._ds(fields)
+        xp, xs, xl = self._cl_field(x)
+        op, os_, ol = self._cl_field(other)
+        shape = self._cl_shape(fields[0])
+        self._check(self.lib.b200seg_cldice_skeleton(xp, None if xs is None else C.cast(xs, _vp), xl, *shape, rounds,
+                                                     fields.data_ptr(), fields.shape[0], op,
+                                                     None if os_ is None else C.cast(os_, _vp), ol, pass_, _p(ws),
+                                                     0 if ws is None else ws.numel() * 8, dev, st))
+
+    def cldice_finalize(self, shape, per_class, labels, alpha, smooth, eps, ws, stats, loss, reduce=True):
+        dev, st = self._ds(stats)
+        self._check(self.lib.b200seg_cldice_finalize(*shape, int(bool(per_class)), int(bool(labels)), _p(alpha),
+                                                     float(smooth), float(eps), int(bool(reduce)), _p(ws),
+                                                     0 if ws is None else ws.numel() * 8, stats.data_ptr(),
+                                                     loss.data_ptr(), dev, st))
+
+    def cldice_bwd(self, x, rounds, fields, grad, scratch, grad_skeleton=None, target=None, target_skeleton=None,
+                   stats=None, gout=None):
+        dev, st = self._ds(grad)
+        _, xs = self._ssim_geom(x)
+        tp, ts, tl = self._cl_field(target)
+        self._check(self.lib.b200seg_cldice_bwd(x.data_ptr(), C.cast(xs, _vp), *self._cl_shape(x), rounds, _p(fields),
+                                                _p(grad_skeleton), tp, None if ts is None else C.cast(ts, _vp), tl,
+                                                _p(target_skeleton), _p(stats), _p(gout), grad.data_ptr(),
+                                                _p(scratch), dev, st))
+
+    def cldice_norm(self, cl, vessel, sums, out):
+        dev, st = self._ds(cl)
+        _, cs = self._ssim_geom(cl)
+        _, vs = self._ssim_geom(vessel)
+        self._check(self.lib.b200seg_cldice_norm(cl.data_ptr(), C.cast(cs, _vp), vessel.data_ptr(), C.cast(vs, _vp),
+                                                 *self._cl_shape(cl), sums.data_ptr(), out.data_ptr(), dev, st))
+
+    def cldice_norm_bwd(self, cl, vessel, sums, gout, grad_cl, grad_vessel):
+        dev, st = self._ds(cl)
+        _, cs = self._ssim_geom(cl)
+        _, vs = self._ssim_geom(vessel)
+        self._check(self.lib.b200seg_cldice_norm_bwd(cl.data_ptr(), C.cast(cs, _vp), vessel.data_ptr(),
+                                                     C.cast(vs, _vp), *self._cl_shape(cl), sums.data_ptr(),
+                                                     gout.data_ptr(), _p(grad_cl), _p(grad_vessel), dev, st))
 
     # ------------------------------------------------------------------ per-step accuracy (model/metric.py)
     def metric_partials(self, probs, labels, threshold, metric):

@@ -164,6 +164,20 @@ int ssim_finalize(int dims, int N, int C, int D, int H, int W, int k, int size_a
 int ssim_bwd(int dims, const float* x, const int64_t* xs, const float* y, const int64_t* ys, int N, int C, int D,
              int H, int W, int k, const float* taps, const double* coef, int size_average, const float* gout,
              const double* acc, float* dx, float* dy, int device, cudaStream_t st);
+int64_t cldice_workspace(int N, int C, int D, int H, int W);
+int cldice_skeleton(const float* x, const int64_t* xs, const int64_t* xlab, int N, int C, int D, int H, int W,
+                    int rounds, float* fields, int nfields, const float* other, const int64_t* os,
+                    const int64_t* olab, int pass, void* ws, long long ws_bytes, int device, cudaStream_t st);
+int cldice_finalize(int N, int C, int D, int H, int W, int per_class, int labels, const float* alpha, double smooth,
+                    double eps, int reduce, const void* ws, long long ws_bytes, double* stats, float* loss,
+                    cudaStream_t st);
+int cldice_bwd(const float* x, const int64_t* xs, int N, int C, int D, int H, int W, int rounds, const float* fields,
+               const float* gsk, const float* t, const int64_t* ts, const int64_t* tlab, const float* skt,
+               const double* stats, const float* gout, float* grad, float* scratch, int device, cudaStream_t st);
+int cldice_norm(const float* cl, const int64_t* cs, const float* v, const int64_t* vs, int N, int C, int D, int H,
+                int W, double* sums, float* r, cudaStream_t st);
+int cldice_norm_bwd(const float* cl, const int64_t* cs, const float* v, const int64_t* vs, int N, int C, int D, int H,
+                    int W, const double* sums, const float* gr, float* gcl, float* gv, int device, cudaStream_t st);
 int cls_head_fwd(const b200seg_tensor* x, const float* w1, const float* b1, const float* w2, const float* b2, int Hd,
                  int K, float* pooled, float* hidden, float* logits, cudaStream_t st);
 int cls_head_bwd(const float* dlogits, const float* pooled, const float* hidden, const float* w1, const float* w2,
@@ -888,6 +902,54 @@ int b200seg_ssim_bwd(int dims, const float* img1, const int64_t* strides1, const
   B200_DEVICE(device);
   return ssim_bwd(dims, img1, strides1, img2, strides2, N, C, D, H, W, window_size, taps, coef, size_average, gout,
                   acc, grad1, grad2, device, ST(stream));
+}
+
+int64_t b200seg_cldice_workspace(int N, int C, int D, int H, int W) {
+  if (N < 1 || C < 1 || D < 1 || H < 1 || W < 1) return 0;
+  return cldice_workspace(N, C, D, H, W);
+}
+
+int b200seg_cldice_skeleton(const float* x, const int64_t* x_strides, const int64_t* x_labels, int N, int C, int D,
+                            int H, int W, int rounds, float* fields, int nfields, const float* other,
+                            const int64_t* other_strides, const int64_t* other_labels, int pass, void* workspace,
+                            int64_t workspace_bytes, int device, b200seg_stream stream) {
+  B200_DEVICE(device);
+  return cldice_skeleton(x, x_strides, x_labels, N, C, D, H, W, rounds, fields, nfields, other, other_strides,
+                         other_labels, pass, workspace, workspace_bytes, device, ST(stream));
+}
+
+int b200seg_cldice_finalize(int N, int C, int D, int H, int W, int per_class, int labels, const float* alpha,
+                            double smooth, double eps, int reduce, const void* workspace, int64_t workspace_bytes,
+                            double* stats, float* loss, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(stats && loss, "b200seg_cldice_finalize: null argument");
+  B200_DEVICE(device);
+  return cldice_finalize(N, C, D, H, W, per_class, labels, alpha, smooth, eps, reduce, workspace, workspace_bytes,
+                         stats, loss, ST(stream));
+}
+
+int b200seg_cldice_bwd(const float* x, const int64_t* x_strides, int N, int C, int D, int H, int W, int rounds,
+                       const float* fields, const float* grad_skeleton, const float* target,
+                       const int64_t* target_strides, const int64_t* target_labels, const float* target_skeleton,
+                       const double* stats, const float* gout, float* grad, float* scratch, int device,
+                       b200seg_stream stream) {
+  B200_DEVICE(device);
+  return cldice_bwd(x, x_strides, N, C, D, H, W, rounds, fields, grad_skeleton, target, target_strides, target_labels,
+                    target_skeleton, stats, gout, grad, scratch, device, ST(stream));
+}
+
+int b200seg_cldice_norm(const float* cl, const int64_t* cl_strides, const float* vessel, const int64_t* vessel_strides,
+                        int N, int C, int D, int H, int W, double* sums, float* out, int device,
+                        b200seg_stream stream) {
+  B200_DEVICE(device);
+  return cldice_norm(cl, cl_strides, vessel, vessel_strides, N, C, D, H, W, sums, out, ST(stream));
+}
+
+int b200seg_cldice_norm_bwd(const float* cl, const int64_t* cl_strides, const float* vessel,
+                            const int64_t* vessel_strides, int N, int C, int D, int H, int W, const double* sums,
+                            const float* gout, float* grad_cl, float* grad_vessel, int device, b200seg_stream stream) {
+  B200_DEVICE(device);
+  return cldice_norm_bwd(cl, cl_strides, vessel, vessel_strides, N, C, D, H, W, sums, gout, grad_cl, grad_vessel,
+                         device, ST(stream));
 }
 
 static bool valid_ratio(const double* r) {
