@@ -373,6 +373,23 @@ int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_
                        const float* coef, const float* seg_scale, const float* gscale, float* dlogits, int device,
                        b200seg_stream stream);
 
+/* ---- binary Lovasz hinge (BinaryLovaszLoss, model/losses.py:235-242 -> model/lovasz.py:35-84), one logit channel.
+ * Over the flattened P = n*vox + v (per_image: per sample n), skipping voxels labelled `ignore` (if has_ignore):
+ * e = 1 - z (t == 1) or 1 + z (t == 0) in fp32, sorted descending (stable: ties in ascending P), grad = Lovasz
+ * gradient of the sorted t (lovasz.py:21-32; no present-class skip: with no foreground grad = (1, 0, ...)), segment
+ * loss = dot(relu(e_sorted), grad), loss = the segment loss, or with per_image the mean over the N samples (a sample
+ * with every voxel ignored adds 0).  Exact integer counts, fp64 Jaccard terms and fixed-order fp64 sums.
+ * logits fp32 [N][vox], labels int64 [N][vox] with values 0, 1 or `ignore`.
+ * b200seg_lovasz_hinge_fwd writes loss, coef [N][vox] = d loss / d logits (0 where ignored or e <= 0) and, if bad is
+ * not null, bad[0] = the number of labels other than 0, 1 and `ignore` (such labels are taken as background).
+ * b200seg_lovasz_hinge_bwd: dlogits = gscale * coef over nvox = N*vox values.  Segments must hold < 2^31 voxels. */
+int64_t b200seg_lovasz_hinge_workspace(int N, int64_t vox_per_sample, int per_image);
+int b200seg_lovasz_hinge_fwd(const float* logits, const int64_t* labels, int N, int64_t vox_per_sample, int per_image,
+                             int has_ignore, int64_t ignore, void* workspace, int64_t workspace_bytes, float* loss,
+                             float* coef, int64_t* bad, int device, b200seg_stream stream);
+int b200seg_lovasz_hinge_bwd(const float* coef, int64_t nvox, const float* gscale, float* dlogits, int device,
+                             b200seg_stream stream);
+
 /* ---- per-step accuracy (model/metric.py:146-181).  b200seg_metric_partials: the sums above from MATERIALISED
  * probabilities (fp32 channels-last [N][vox][C], threshold 0.5 in the reference); b200seg_metric_finalize:
  * out[0] = dice_coeff (C == 1) / multiclass_dice_coeff (mean over classes 1..C-1), out[1] = the iou_coeff analogue. */

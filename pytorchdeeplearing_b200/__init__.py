@@ -1,7 +1,8 @@
 """pytorchdeeplearing_b200 -- H100-native (sm_90a) drop-in for the segmentation hot path of
 junqiangchen/PytorchDeepLearing: ``networks/VNet3d.py``, ``networks/Unet3d.py``,
 ``networks/Unet3dthin.py``, ``networks/Unet2d.py`` forward/backward, the ``networks/ResNet3d.py`` / ``ResNet2d.py`` classifiers and the losses of ``model/losses.py`` (Dice / BCE / focal / CE,
-Jaccard / Tversky / sensitivity-specificity / exponential-log Dice and Lovasz-Softmax) (SURVEY.md section 8), and the
+Jaccard / Tversky / sensitivity-specificity / exponential-log Dice, Lovasz-Softmax and the binary Lovasz hinge)
+(SURVEY.md section 8), and the
 3-D evaluation metrics of ``model/metric.py`` (``Seg_Metirc3d``, ``seg_metrics3d``) and the SSIM losses of
 ``model/lossesSSIM.py`` (``SSIM``, ``SSIM3D``, ``ssim``, ``ssim3D``), the soft-clDice losses of ``model/lossescldice.py``
 (``soft_skeletonize``, ``norm_intersection``, ``Binary_Soft_cldice_loss``, ``Mutil_Soft_cldice_loss``; the reference
@@ -23,7 +24,7 @@ from .networks import VNet3d, VNet2d, UNet3d, UNet3dthin, UNet2d, ResNet3d, ResN
 from .losses import (BinaryDiceLoss, BinaryCrossEntropyLoss, BinaryFocalLoss, BinaryCrossEntropyDiceLoss,
                      BinaryDiceFocalLoss, MutilCrossEntropyLoss, MutilFocalLoss, MutilDiceLoss,
                      MutilCrossEntropyDiceLoss, BinaryJaccardLoss, BinaryELDiceLoss, BinarySSLoss, BinaryTverskyLoss,
-                     MutilELDiceLoss, LovaszLoss)
+                     MutilELDiceLoss, LovaszLoss, BinaryLovaszLoss, lovasz_hinge)
 from .install import install, uninstall
 from .graphed import GraphedStep
 from .optim import FusedAdamW, FusedAdam
@@ -43,5 +44,5 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
            "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
-           "MutilELDiceLoss", "LovaszLoss", "SSIM", "SSIM3D", "ssim", "ssim3D",
+           "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge", "SSIM", "SSIM3D", "ssim", "ssim3D",
            "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss"]

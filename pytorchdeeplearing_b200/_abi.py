@@ -113,6 +113,9 @@ _SIGNATURES = {
     "b200seg_lovasz_workspace": ([_i, _i64, _i, _i], C.c_int64),
     "b200seg_lovasz_fwd": ([_vp, _vp, _i, _i64, _i, _i, _i, _i64, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_lovasz_bwd": ([_vp, _vp, _i, _i64, _i, _i, _vp, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_lovasz_hinge_workspace": ([_i, _i64, _i], C.c_int64),
+    "b200seg_lovasz_hinge_fwd": ([_vp, _vp, _i, _i64, _i, _i, _i64, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_lovasz_hinge_bwd": ([_vp, _i64, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_segmetric3d_workspace": ([_i, _i, _i, _i], C.c_int64),
     "b200seg_segmetric3d": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _i, _vp], C.c_int),
     "b200seg_segmetric3d_points": ([_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp,
@@ -799,6 +802,24 @@ class CudaBackend:
         self._check(self.lib.b200seg_lovasz_bwd(logits.data_ptr(), labels.data_ptr(), n, logits.numel() // (n * c), c,
                                                 1 if per_image else 0, coef.data_ptr(), seg_scale.data_ptr(),
                                                 gscale.data_ptr(), dlogits.data_ptr(), dev, st))
+
+    def lovasz_hinge_fwd(self, logits, labels, per_image, ignore, loss, coef, bad=None):
+        """logits (N, ..., 1) fp32 contiguous, labels int64 with N*vox elements; coef like logits (d loss / d logits);
+        bad: None or int64 [1] (labels other than 0, 1 and ignore).  ignore: None or an int label value"""
+        dev, st = self._ds(logits)
+        n = logits.shape[0]
+        vox = logits.numel() // n
+        nb = int(self.lib.b200seg_lovasz_hinge_workspace(n, vox, 1 if per_image else 0))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=logits.device)
+        self._check(self.lib.b200seg_lovasz_hinge_fwd(logits.data_ptr(), labels.data_ptr(), n, vox,
+                                                      1 if per_image else 0, 0 if ignore is None else 1,
+                                                      0 if ignore is None else int(ignore), ws.data_ptr(), nb,
+                                                      loss.data_ptr(), coef.data_ptr(), _p(bad), dev, st))
+
+    def lovasz_hinge_bwd(self, coef, gscale, dlogits):
+        dev, st = self._ds(coef)
+        self._check(self.lib.b200seg_lovasz_hinge_bwd(coef.data_ptr(), coef.numel(), gscale.data_ptr(),
+                                                      dlogits.data_ptr(), dev, st))
 
     # ------------------------------------------------------------------ 3-D segmentation metrics (model/metric.py:11-142)
     _MASK_DTYPES = {torch.bool: U8, torch.uint8: U8, torch.int32: I32, torch.int64: I64}

@@ -147,6 +147,11 @@ int lovasz_fwd(const float* z, const long long* t, int N, long long vox, int C, 
                cudaStream_t s);
 int lovasz_bwd(const float* z, const long long* t, int N, long long vox, int C, int per_image, const float* coef,
                const float* seg_scale, const float* gscale, float* dz, int device, cudaStream_t s);
+int64_t lovasz_hinge_workspace(int N, long long vox, int per_image);
+int lovasz_hinge_fwd(const float* z, const long long* t, int N, long long vox, int per_image, int has_ignore,
+                     long long ignore, void* ws, long long ws_bytes, float* loss, float* coef, long long* bad,
+                     int device, cudaStream_t s);
+int lovasz_hinge_bwd(const float* coef, long long total, const float* gscale, float* dz, int device, cudaStream_t s);
 int64_t segmetric3d_workspace(int N, int D, int H, int W);
 int segmetric3d(const void* real, int rdt, const void* pred, int pdt, int N, int D, int H, int W,
                 const double* spacing, void* ws, long long ws_bytes, long long* counts, double* metrics, int* flags,
@@ -839,6 +844,28 @@ int b200seg_lovasz_bwd(const float* logits, const int64_t* labels, int N, int64_
   B200_DEVICE(device);
   return lovasz_bwd(logits, reinterpret_cast<const long long*>(labels), N, vox, C, per_image, coef, seg_scale, gscale,
                     dlogits, device, ST(stream));
+}
+
+int64_t b200seg_lovasz_hinge_workspace(int N, int64_t vox, int per_image) {
+  if (N < 1 || vox < 1) return 0;
+  return lovasz_hinge_workspace(N, vox, per_image);
+}
+
+int b200seg_lovasz_hinge_fwd(const float* logits, const int64_t* labels, int N, int64_t vox, int per_image,
+                             int has_ignore, int64_t ignore, void* workspace, int64_t workspace_bytes, float* loss,
+                             float* coef, int64_t* bad, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(logits && labels && loss && coef, "b200seg_lovasz_hinge_fwd: null argument");
+  B200_DEVICE(device);
+  return lovasz_hinge_fwd(logits, reinterpret_cast<const long long*>(labels), N, vox, per_image, has_ignore, ignore,
+                          workspace, workspace_bytes, loss, coef, reinterpret_cast<long long*>(bad), device,
+                          ST(stream));
+}
+
+int b200seg_lovasz_hinge_bwd(const float* coef, int64_t nvox, const float* gscale, float* dlogits, int device,
+                             b200seg_stream stream) {
+  B200_CHECK_ARG(coef && gscale && dlogits, "b200seg_lovasz_hinge_bwd: null argument");
+  B200_DEVICE(device);
+  return lovasz_hinge_bwd(coef, nvox, gscale, dlogits, device, ST(stream));
 }
 
 int64_t b200seg_segmetric3d_workspace(int N, int D, int H, int W) {

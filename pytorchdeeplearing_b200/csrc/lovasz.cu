@@ -476,4 +476,245 @@ int lovasz_bwd(const float* z, const long long* t, int N, long long vox, int C, 
   return B200SEG_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ binary Lovasz hinge
+// BinaryLovaszLoss (model/losses.py:235-242 -> model/lovasz.py:35-84) on the same sort.  One segment (all N*vox
+// logits) or one per sample (per_image).  e = 1 - z (t == 1) or 1 + z (t == 0), as fp32 forms 1 - z * (2t - 1).
+// Elements with e <= 0 add nothing to the loss (relu), get no gradient and, sorted after every e > 0, change no
+// Jaccard term of an element before them; so they take the ignored key and the sort is the Lovasz-Softmax one.  gts,
+// the foreground count of the Jaccard terms, still counts every valid foreground voxel: it comes from the labels.
+__global__ void __launch_bounds__(kThreads) hinge_keys_kernel(const float* __restrict__ z,
+                                                              const long long* __restrict__ t, long long len,
+                                                              int has_ignore, long long ignore,
+                                                              uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+  PDL_ENTER();
+  const long long p0 = (long long)blockIdx.y * len;
+  uint32_t* k = keys + p0;
+  int32_t* v = vals + p0;
+  for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j < len;
+       j += (long long)gridDim.x * blockDim.x) {
+    const long long lbl = t[p0 + j];
+    const float zz = z[p0 + j];
+    const float e = lbl == 1 ? 1.f - zz : 1.f + zz;      // lovasz.py:63-64 (a NaN e keeps a key and gives a NaN loss)
+    const bool dropped = (has_ignore && lbl == ignore) || e <= 0.f;
+    k[j] = dropped ? kIgnoredKey : (~__float_as_uint(e)) & 0x7FFFFFFFu;
+    v[j] = (int32_t)j;
+  }
+}
+
+// per sorted tile: cnt[0] = foreground with e > 0 (the prefix counts), cnt[1] = valid foreground (gts), cnt[2] = valid
+// labels other than 0 and 1; cnt[q] at [(q*nseg + s)*ntiles + tile]
+__global__ void __launch_bounds__(kThreads) hinge_tilecnt_kernel(const uint32_t* __restrict__ keys,
+                                                                 const int32_t* __restrict__ vals,
+                                                                 const long long* __restrict__ t, long long len,
+                                                                 int ntiles, int has_ignore, long long ignore,
+                                                                 uint32_t* __restrict__ cnt) {
+  PDL_ENTER();
+  __shared__ unsigned long long s_tmp[kWarps];
+  const int seg = blockIdx.y, nseg = gridDim.y;
+  const long long p0 = (long long)seg * len;
+  const uint32_t* k = keys + p0;
+  const int32_t* v = vals + p0;
+  const long long t0 = (long long)blockIdx.x * kTile;
+  unsigned long long npos = 0, nfg = 0, nbad = 0;
+  for (int i = threadIdx.x; i < kTile; i += kThreads) {
+    const long long j = t0 + i;
+    if (j >= len) break;
+    const long long lbl = t[p0 + v[j]];
+    if (has_ignore && lbl == ignore) continue;
+    nfg += lbl == 1;
+    npos += lbl == 1 && k[j] != kIgnoredKey;
+    nbad += lbl != 0 && lbl != 1;
+  }
+  npos = block_sum_u64(npos, s_tmp);
+  nfg = block_sum_u64(nfg, s_tmp);
+  nbad = block_sum_u64(nbad, s_tmp);
+  if (threadIdx.x == 0) {
+    const long long o = (long long)seg * ntiles + blockIdx.x, q = (long long)nseg * ntiles;
+    cnt[o] = (uint32_t)npos;
+    cnt[q + o] = (uint32_t)nfg;
+    cnt[2 * q + o] = (uint32_t)nbad;
+  }
+}
+
+// Lovasz gradient of the sorted segment (lovasz.py:21-32) as lovasz_grad_kernel, with gts from cnt[1] and J_{-1} = 0
+// (gts = 0 gives J = 1 everywhere, so grad = (1, 0, 0, ...)).  coef = d loss / d z = -(2t - 1) grad / nimg in one
+// rounding (0 for dropped elements); tileloss = sum relu(e) grad over the tile.
+__global__ void __launch_bounds__(kThreads) hinge_grad_kernel(const uint32_t* __restrict__ keys,
+                                                              const int32_t* __restrict__ vals,
+                                                              const long long* __restrict__ t, long long len,
+                                                              int ntiles, const uint32_t* __restrict__ cnt,
+                                                              float* __restrict__ coef, double* __restrict__ tileloss) {
+  PDL_ENTER();
+  __shared__ uint32_t s_warp[kWarps];
+  __shared__ unsigned long long s_u[kWarps];
+  __shared__ double s_d[kWarps];
+  const int seg = blockIdx.y, nseg = gridDim.y;
+  const long long p0 = (long long)seg * len;
+  const uint32_t* k = keys + p0;
+  const int32_t* v = vals + p0;
+  const uint32_t* cpos = cnt + (long long)seg * ntiles;
+  const uint32_t* cfg = cpos + (long long)nseg * ntiles;
+  unsigned long long before = 0, all = 0;
+  for (int i = threadIdx.x; i < ntiles; i += kThreads) {
+    all += cfg[i];
+    if (i < (int)blockIdx.x) before += cpos[i];
+  }
+  before = block_sum_u64(before, s_u);
+  const double g = (double)block_sum_u64(all, s_u);
+  const double inv_nimg = 1.0 / (double)nseg;
+  const long long j0 = (long long)blockIdx.x * kTile + (long long)threadIdx.x * kItems;
+  uint32_t kk[kItems];
+  int32_t vv[kItems];
+  unsigned fgbits = 0;
+  uint32_t mine = 0;
+#pragma unroll
+  for (int q = 0; q < kItems; ++q) {
+    const long long j = j0 + q;
+    kk[q] = kIgnoredKey;
+    vv[q] = 0;
+    if (j < len) {
+      kk[q] = k[j];
+      vv[q] = v[j];
+      if (kk[q] != kIgnoredKey && t[p0 + vv[q]] == 1) {
+        fgbits |= 1u << q;
+        ++mine;
+      }
+    }
+  }
+  uint32_t tot;
+  const uint32_t ex = block_exclusive_scan(mine, s_warp, &tot);
+  long long cum = (long long)before + ex;
+  double acc = 0.0;
+#pragma unroll
+  for (int q = 0; q < kItems; ++q) {
+    const long long j = j0 + q;
+    if (j >= len) break;
+    const int fg = (fgbits >> q) & 1;
+    cum += fg;
+    float d = 0.f;
+    if (kk[q] != kIgnoredKey) {
+      const double cf = (double)cum, cp = (double)(cum - fg);
+      const double Ji = 1.0 - (g - cf) / (g + ((double)(j + 1) - cf));
+      const double Jp = j == 0 ? 0.0 : 1.0 - (g - cp) / (g + ((double)j - cp));
+      const double gr = Ji - Jp;
+      acc += (double)__uint_as_float(~kk[q] & 0x7FFFFFFFu) * gr;
+      d = (float)((fg ? -gr : gr) * inv_nimg);
+    }
+    coef[p0 + vv[q]] = d;
+  }
+  acc = block_sum(acc, s_d);
+  if (threadIdx.x == 0) tileloss[(long long)seg * ntiles + blockIdx.x] = acc;
+}
+
+// loss = (sum over segments of the segment loss) / nimg, each segment summed over its tiles in a fixed order;
+// bad[0] = labels other than 0, 1 and ignore.  One block.
+__global__ void __launch_bounds__(kThreads) hinge_finalize_kernel(const uint32_t* __restrict__ cnt,
+                                                                  const double* __restrict__ tileloss, int nseg,
+                                                                  int ntiles, float* __restrict__ loss,
+                                                                  long long* __restrict__ bad) {
+  PDL_ENTER();
+  __shared__ unsigned long long s_u[kWarps];
+  __shared__ double s_d[kWarps];
+  double total = 0.0;
+  unsigned long long nbad = 0;
+  const uint32_t* cbad = cnt + 2LL * nseg * ntiles;
+  for (int s = 0; s < nseg; ++s) {
+    double l = 0.0;
+    for (int i = threadIdx.x; i < ntiles; i += kThreads) {
+      l += tileloss[(long long)s * ntiles + i];
+      nbad += cbad[(long long)s * ntiles + i];
+    }
+    total += block_sum(l, s_d);
+  }
+  nbad = block_sum_u64(nbad, s_u);
+  if (threadIdx.x == 0) {
+    loss[0] = (float)(total / nseg);
+    if (bad) bad[0] = (long long)nbad;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) hinge_bwd_kernel(const float* __restrict__ coef, long long total,
+                                                             const float* __restrict__ gscale, float* __restrict__ dz) {
+  PDL_ENTER();
+  const float gs = gscale[0];
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x)
+    dz[i] = gs * coef[i];
+}
+
+namespace {
+struct HingeLayout {
+  int nseg, ntiles;
+  long long len;
+  size_t off_ka, off_va, off_kb, off_vb, off_sort, off_cnt, off_loss, bytes;
+};
+
+HingeLayout hinge_layout(int N, long long vox, int per_image) {
+  HingeLayout L;
+  L.nseg = per_image ? N : 1;
+  L.len = per_image ? vox : (long long)N * vox;
+  L.ntiles = (int)tiles_of(L.len);
+  const size_t pairs = (size_t)L.nseg * (size_t)L.len;
+  size_t o = 0;
+  L.off_ka = o; o += align256(pairs * 4);
+  L.off_va = o; o += align256(pairs * 4);
+  L.off_kb = o; o += align256(pairs * 4);
+  L.off_vb = o; o += align256(pairs * 4);
+  L.off_sort = o; o += (size_t)radix_sort_workspace(L.nseg, L.len);
+  L.off_cnt = o; o += align256((size_t)3 * L.nseg * L.ntiles * 4);
+  L.off_loss = o; o += align256((size_t)L.nseg * L.ntiles * 8);
+  L.bytes = o;
+  return L;
+}
+}  // namespace
+
+int64_t lovasz_hinge_workspace(int N, long long vox, int per_image) {
+  return (int64_t)hinge_layout(N, vox, per_image).bytes;
+}
+
+int lovasz_hinge_fwd(const float* z, const long long* t, int N, long long vox, int per_image, int has_ignore,
+                     long long ignore, void* ws, long long ws_bytes, float* loss, float* coef, long long* bad,
+                     int device, cudaStream_t s) {
+  B200_CHECK_ARG(N >= 1 && vox >= 1, "lovasz_hinge: empty batch");
+  const HingeLayout L = hinge_layout(N, vox, per_image);
+  B200_CHECK_ARG(L.len < (1LL << 31), "lovasz_hinge: a segment of %lld voxels (at most 2^31 - 1)", L.len);
+  B200_CHECK_ARG(L.nseg <= 65535, "lovasz_hinge: %d samples per image (at most 65535)", L.nseg);
+  B200_CHECK_ARG(ws && (size_t)ws_bytes >= L.bytes, "lovasz_hinge: workspace too small");
+  char* w = static_cast<char*>(ws);
+  uint32_t* ka = reinterpret_cast<uint32_t*>(w + L.off_ka);
+  int32_t* va = reinterpret_cast<int32_t*>(w + L.off_va);
+  uint32_t* kb = reinterpret_cast<uint32_t*>(w + L.off_kb);
+  int32_t* vb = reinterpret_cast<int32_t*>(w + L.off_vb);
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(w + L.off_cnt);
+  double* tl = reinterpret_cast<double*>(w + L.off_loss);
+  long long kb_x = (L.len + kThreads * 4 - 1) / (kThreads * 4);
+  const long long cap = ((long long)num_sms(device) * 8 + L.nseg - 1) / L.nseg;
+  if (kb_x > cap) kb_x = cap;
+  if (kb_x < 1) kb_x = 1;
+  launch_k(hinge_keys_kernel, dim3((unsigned)kb_x, L.nseg), kThreads, 0, s, z, t, L.len, has_ignore, ignore, ka, va);
+  B200_LAUNCH_CHECK();
+  const int rc = radix_sort_pairs(ka, va, kb, vb, L.nseg, L.len, w + L.off_sort, (long long)(L.off_cnt - L.off_sort),
+                                  s);
+  if (rc != B200SEG_OK) return rc;
+  const dim3 grid(L.ntiles, L.nseg);
+  launch_k(hinge_tilecnt_kernel, grid, kThreads, 0, s, (const uint32_t*)kb, (const int32_t*)vb, t, L.len, L.ntiles,
+           has_ignore, ignore, cnt);
+  launch_k(hinge_grad_kernel, grid, kThreads, 0, s, (const uint32_t*)kb, (const int32_t*)vb, t, L.len, L.ntiles,
+           (const uint32_t*)cnt, coef, tl);
+  launch_k(hinge_finalize_kernel, 1, kThreads, 0, s, (const uint32_t*)cnt, (const double*)tl, L.nseg, L.ntiles, loss,
+           bad);
+  B200_LAUNCH_CHECK();
+  return B200SEG_OK;
+}
+
+int lovasz_hinge_bwd(const float* coef, long long total, const float* gscale, float* dz, int device, cudaStream_t s) {
+  B200_CHECK_ARG(total >= 1, "lovasz_hinge_bwd: empty batch");
+  long long blocks = (total + kThreads * 4 - 1) / (kThreads * 4);
+  const long long cap = (long long)num_sms(device) * 8;
+  if (blocks > cap) blocks = cap;
+  launch_k(hinge_bwd_kernel, (unsigned)blocks, kThreads, 0, s, coef, total, gscale, dz);
+  B200_LAUNCH_CHECK();
+  return B200SEG_OK;
+}
+
 }  // namespace b200seg

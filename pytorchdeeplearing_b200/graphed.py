@@ -35,7 +35,8 @@ import torch
 
 from . import runtime
 from .engine import Engine
-from .losses import LOVASZ, SS, ignore_label, loss_spec, lovasz_check, lovasz_scale_size, prepare_labels
+from .losses import (LOVASZ, LOVASZ_HINGE, SS, _check_labels_default, ignore_label, loss_spec, lovasz_check,
+                     lovasz_hinge_bad_labels, lovasz_hinge_check, lovasz_scale_size, prepare_labels)
 
 
 def _is_fused_optimizer(opt) -> bool:
@@ -63,7 +64,11 @@ class GraphedStep:
         if self._terms == LOVASZ:
             lovasz_check(c)
             self._per_image, self._ignore = bool(lossfn.per_image), ignore_label(lossfn.ignore)
+        elif self._terms == LOVASZ_HINGE:
+            lovasz_hinge_check(c, y0)
+            self._per_image, self._ignore = bool(lossfn.per_image), ignore_label(lossfn.ignore_index)
         dev = self.x.device
+        self._bad = torch.zeros(1, dtype=torch.int64, device=dev) if self._terms == LOVASZ_HINGE else None
         self._one = torch.ones(1, dtype=torch.float32, device=dev)
         # class weights of the loss: a constant of the step, created once (not a fill launch inside every step)
         self._alpha_t = torch.ones(c, dtype=torch.float32, device=dev) if self._alpha is None else \
@@ -78,6 +83,8 @@ class GraphedStep:
         self.loss = self.dice = self.probs = None
         for _ in range(max(1, warmup)):
             self._eager_step()
+        if self._terms == LOVASZ_HINGE and _check_labels_default():
+            self.check_labels()
         if self.use_graph:
             self._capture()
 
@@ -151,6 +158,10 @@ class GraphedStep:
             scale = torch.empty(lovasz_scale_size(z.shape[0], c, self._per_image), dtype=torch.float32, device=dev)
             be.lovasz_fwd(z, self.y, self._per_image, self._ignore, loss, coef, scale)
             be.lovasz_bwd(z, self.y, self._per_image, coef, scale, self._one, dz)
+        elif self._terms == LOVASZ_HINGE:
+            coef = torch.empty_like(z)
+            be.lovasz_hinge_fwd(z, self.y, self._per_image, self._ignore, loss, coef, self._bad)
+            be.lovasz_hinge_bwd(coef, self._one, dz)
         else:
             lcoef = torch.empty(2 * c + 3 if c > 1 else 5, dtype=torch.float32, device=dev)
             be.loss_finalize(part, c, self._terms, self._alpha_t, self._gamma, self._alpha_f, loss, lcoef)
@@ -320,8 +331,11 @@ class GraphedStep:
     def check_labels(self) -> None:
         """Raise if the last step saw a label outside [0, numclass) (the reference raises in F.one_hot /
         F.cross_entropy; a captured step cannot, so the loss becomes NaN and this check names the cause).
-        Synchronises.  LovaszLoss takes such labels as background (the reference does not raise there)."""
-        if self.ncls > 1 and self._terms != LOVASZ:
+        Synchronises.  LovaszLoss takes such labels as background (the reference does not raise there).
+        BinaryLovaszLoss: raise ValueError if the last step saw a label other than 0, 1 and ignore_index."""
+        if self._terms == LOVASZ_HINGE:
+            lovasz_hinge_bad_labels(self._bad)
+        elif self.ncls > 1 and self._terms != LOVASZ:
             bad = int(self._part[-1].item())
             if bad:
                 raise RuntimeError(f"{bad} label value(s) outside [0, {self.ncls})")

@@ -21,7 +21,7 @@ _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "B
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
 # the further model/losses.py classes (bound there, not imported by the wrappers)
 _EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss", "MutilELDiceLoss",
-                   "LovaszLoss")
+                   "LovaszLoss", "BinaryLovaszLoss")
 # model/lossesSSIM.py
 _SSIM_NAMES = ("SSIM", "SSIM3D", "ssim", "ssim3D")
 # model/lossescldice.py

@@ -20,6 +20,7 @@ from . import runtime
 DICE, CE, FOCAL = 1, 2, 4
 JACCARD, ELDICE, TVERSKY, SS = 8, 16, 32, 64     # include/b200seg.h B200SEG_LOSS_*: each one alone
 LOVASZ = 128                                     # not a finalize term: the sort-based Lovasz-Softmax path
+LOVASZ_HINGE = 256                               # not a finalize term: the sort-based binary Lovasz hinge path
 
 
 def _check_labels_default() -> bool:
@@ -176,6 +177,63 @@ class _LovaszLoss(torch.autograd.Function):
         return logits_grad(dz, ctx.perm), None, None, None, None
 
 
+def lovasz_hinge_check(c: int, labels: torch.Tensor) -> None:
+    """what BinaryLovaszLoss refuses: more than one logit channel, floating-point labels, data parallelism"""
+    if c != 1:
+        raise ValueError(f"BinaryLovaszLoss takes logits of one channel, got {c}")
+    if labels.is_floating_point():
+        raise TypeError(f"BinaryLovaszLoss takes integer labels 0 / 1 (or ignore_index), got {labels.dtype}")
+    if runtime.dp_state()[0]:
+        raise RuntimeError("BinaryLovaszLoss does not run under data parallelism: its value on the global batch needs "
+                           "one sort over every rank's voxels")
+
+
+def lovasz_hinge_bad_labels(bad: torch.Tensor) -> None:
+    """raise if the hinge's label count found values other than 0, 1 and ignore_index (synchronises)"""
+    n = int(bad.item())
+    if n:
+        raise ValueError(f"{n} label value(s) other than 0 and 1: BinaryLovaszLoss takes binary labels "
+                         "(or ignore_index)")
+
+
+class _LovaszHingeLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, labels, per_image, ignore, owner):
+        if logits.dim() not in (2, 4, 5):
+            raise ValueError(f"BinaryLovaszLoss takes (N, 1), (N, 1, H, W) or (N, 1, D, H, W) logits, got "
+                             f"{tuple(logits.shape)}")
+        lovasz_hinge_check(logits.shape[1], labels)
+        be = runtime.get_backend(logits)
+        z, perm = prepare_logits(logits)
+        t = prepare_labels(labels, 1)
+        if t.numel() != z.numel():
+            raise RuntimeError(f"label shape {tuple(labels.shape)} does not match logits {tuple(logits.shape)}")
+        dev, n = z.device, z.shape[0]
+        buf = torch.zeros(be.part_size(1) + n * 3, dtype=torch.float64, device=dev)
+        metric = buf[be.part_size(1):].view(n, 1, 3)
+        be.loss_partials(z, t, 2.0, 0.25, buf[:be.part_size(1)], metric)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        coef = torch.empty_like(z)
+        bad = torch.empty(1, dtype=torch.int64, device=dev)
+        be.lovasz_hinge_fwd(z, t, per_image, ignore_label(ignore), loss, coef, bad)
+        if _check_labels_default() and not runtime.is_capturing(dev):
+            lovasz_hinge_bad_labels(bad)
+        if owner is not None:
+            owner._metric_sums = metric
+        ctx.save_for_backward(coef)
+        ctx.perm = perm
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        coef, = ctx.saved_tensors
+        be = runtime.get_backend(coef)
+        dz = torch.empty_like(coef)
+        g = gout.detach().to(torch.float32).reshape(1).contiguous()
+        be.lovasz_hinge_bwd(coef, g, dz)
+        return logits_grad(dz, ctx.perm), None, None, None, None
+
+
 class _LossBase(nn.Module):
     """Common part of the loss modules: after every ``forward`` the per-sample sums of the reference's per-step
     accuracy (model/metric.py:146-181) are available from the SAME pass over logits + labels."""
@@ -205,7 +263,8 @@ def loss_spec(lossfn):
              "MutilCrossEntropyLoss": CE, "MutilFocalLoss": FOCAL, "MutilDiceLoss": DICE,
              "MutilCrossEntropyDiceLoss": DICE | CE,
              "BinaryJaccardLoss": JACCARD, "BinaryELDiceLoss": ELDICE, "BinaryTverskyLoss": TVERSKY,
-             "BinarySSLoss": SS, "MutilELDiceLoss": ELDICE, "LovaszLoss": LOVASZ}
+             "BinarySSLoss": SS, "MutilELDiceLoss": ELDICE, "LovaszLoss": LOVASZ,
+             "BinaryLovaszLoss": LOVASZ_HINGE}
     if name not in table:
         raise TypeError(f"{name} is not a pytorchdeeplearing_b200 loss")
     alpha = getattr(lossfn, "alpha", None) if name.startswith("Mutil") and (table[name] & (DICE | ELDICE)) else None
@@ -397,7 +456,27 @@ class LovaszLoss(_LossBase):
         return _LovaszLoss.apply(logits, target, bool(self.per_image), self.ignore, self)
 
 
+class BinaryLovaszLoss(_LossBase):
+    """reference model/losses.py:235-242 -> model/lovasz.py:35-84 (binary Lovasz hinge on one logit channel).  The
+    reference's constructor never runs nn.Module.__init__ (an unbound super), so its objects cannot be called; this one
+    can.  Labels must be integer 0 / 1 or ``ignore_index``; a sample with every voxel ignored adds 0 (with per_image,
+    it still counts in the mean).  Not available under data parallelism (it needs a global sort)."""
+
+    def __init__(self, per_image: bool = False, ignore_index=None):
+        super().__init__()
+        self.ignore_index = ignore_index
+        self.per_image = per_image
+
+    def forward(self, logits, target):
+        return _LovaszHingeLoss.apply(logits, target, bool(self.per_image), self.ignore_index, self)
+
+
+def lovasz_hinge(logits, labels, per_image=True, ignore_index=None):
+    """model/lovasz.py:35-50 ``_lovasz_hinge`` (its defaults) on the logit layouts of BinaryLovaszLoss"""
+    return _LovaszHingeLoss.apply(logits, labels, bool(per_image), ignore_index, None)
+
+
 __all__ = ["BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
            "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
-           "MutilELDiceLoss", "LovaszLoss"]
+           "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge"]
