@@ -212,8 +212,8 @@ def wgrad_a_spatial(ws):
 
 # ---------------------------------------------------------------------------------------------------------- operands
 def grid(shape, k, e, gen):
-    """integers in [-k, k] times 2^-e (bf16-exact for k <= 256)"""
-    return torch.randint(-k, k + 1, shape, generator=gen).double() * 2.0 ** -e
+    """integers in [-k, k] times 2^-e (bf16-exact for k <= 256), on the generator's device"""
+    return torch.randint(-k, k + 1, shape, generator=gen, device=gen.device).double() * 2.0 ** -e
 
 
 def conv_operands(cs, seed=0):
@@ -282,22 +282,45 @@ def assert_bitwise(got, want, what):
     assert msg is None, f"{what}: {msg}"
 
 
-def stats_chain(path, n, ys, cout, up=False):
+def stats_chain(path, n, ys, cout, up=False, kind=K3, dims=3, sms=SMS):
     """L: an upper bound on the number of fp32 additions any value passes through on its way into a [n][c] statistic.
     HALO3 / HALO_WS (conv_halo.cu, conv_halo_ws.cu): a per-thread chain over the slices of one column segment (<= D),
     a 5-level warp butterfly, then one addition into the warp's shared-memory row per segment of the CTA's range
     (<= units per CTA); the four warp rows and the flushes are added in fp64.  TC / PW_MMA (conv_tc.cu, pw_mma.cu):
     a per-tile butterfly, then one addition per tile into the warp's row (<= tiles per sample).  PW_MMA (pw_mma.cu):
     a per-thread chain of 8 additions per tap per 512-voxel tile of the CTA's range (2 CTAs per SM, 1 for UP), a
-    3-level butterfly; the eight warp rows are added in fp64."""
+    3-level butterfly; the eight warp rows are added in fp64.
+    GENERIC (conv_generic.cu:186-216): each thread adds the (at most) 4 rows it owns of one output column in fp32
+    (s += v, q = fmaf(v, v, q)); the BM/4 row partials of a CTA and the CTAs' atomics are fp64.
+    STEM (stem.cu:99-128, grid stem.cu:253-259): a per-thread fp32 chain over its VPT voxels of every item of its
+    grid-stride range (grid <= 2 SMs / N CTAs per sample, 256 threads), then a 5-level warp butterfly; the 8 warp
+    rows and the atomics are fp64.  SMALLCIN (small_channels.cu:77-103, grid :347-350): the same with one voxel per
+    item and a grid of <= 8 SMs / N CTAs per sample.  STEM_MMA (stem_mma.cu:74-99, 146-153, grid stem_mma.cuh:131):
+    two fp32 additions per 16-column segment of each 8-row tile of the CTA's range (tiles * segments per sample =
+    D H/8 W/16, <= 8 segments per tile, one CTA per tile up to 2 SMs), flushed at each new sample, then a 3-level
+    butterfly; the 8 warp rows and the atomics are fp64."""
     d, h, w = ys
     if path in ("HALO3", "HALO_WS"):
         units = n * d * -(-h // 16) * -(-w // 8) * (cout // 64 if path == "HALO_WS" else 1)
-        return d + 6 + -(-units // min(units, SMS))
+        return d + 6 + -(-units // min(units, sms))
     if path == "PW_MMA":
         taps = 8 if up else 1
         tiles = n * d * h * w // taps // 512
-        return -(-tiles // min(tiles, SMS * (1 if up else 2))) * 8 * taps + 4
+        return -(-tiles // min(tiles, sms * (1 if up else 2))) * 8 * taps + 4
+    if path == "GENERIC":
+        return 4
+    if path == "STEM":
+        vpt = 2 if (kind == K1 or dims == 2) and w % 2 == 0 else 1
+        items = d * h * (w // vpt)
+        grid_ = min(-(-items // 256), -(-2 * sms // n))
+        return vpt * -(-items // (grid_ * 256)) + 5
+    if path == "SMALLCIN":
+        v = d * h * w
+        grid_ = min(-(-v // 256), -(-8 * sms // n))
+        return -(-v // (grid_ * 256)) + 5
+    if path == "STEM_MMA":
+        segs = n * d * (h // 8) * (w // 16)
+        return 2 * (-(-segs // (2 * sms)) + 8) + 3
     return 6 + -(-d * h * w // 64)
 
 
@@ -516,6 +539,33 @@ def test_conv_exact_sees_swapped_taps(be):
     assert first_mismatch(gy.view.cpu(), y.float().bfloat16()) is not None
 
 
+def bwdstats_want(g_bf, yf, stats, gamma, beta, scale, groups, eps, chain):
+    """fp64 {sum g m, sum g m yfwd} per (n, c) and their bounds (s0, t0, s1, t1).  m is the ReLU mask from A, B derived
+    in fp64 as the kernels' load_coefs does (group mean / rstd from the statistics, rounded to fp32); scale None is
+    no dropout.  The bound is an fp32 chain of at most `chain` additions plus every term whose z is within 2^-20 of
+    the threshold (there the fp32 fmaf may take either side)."""
+    n, co = yf.shape[0], yf.shape[-1]
+    vox = yf[0, ..., 0].numel()
+    cpg = co // groups
+    st = stats.view(n, groups, cpg, 2).sum(2)
+    m_ = float(cpg * vox)
+    mean = st[..., 0] / m_
+    var = (st[..., 1] / m_ - mean * mean).clamp_min(0)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    mean_c, rstd_c = mean.repeat_interleave(cpg, 1), rstd.repeat_interleave(cpg, 1)
+    s = 1.0 if scale is None else scale.double()
+    A = (rstd_c * gamma.double() * s).float().double().view(n, 1, 1, 1, co)
+    B = ((beta.double() - mean_c * rstd_c * gamma.double()) * s).float().double().view(n, 1, 1, 1, co)
+    z = yf * A + B
+    amb = z.abs() <= 2.0 ** -20 * ((yf * A).abs() + B.abs())
+    m = (z > 0).double()
+    gd = g_bf.double()
+    s0, s1 = (gd * m).sum((1, 2, 3)), (gd * m * yf).sum((1, 2, 3))
+    t0 = 2.0 ** -24 * chain * gd.abs().sum((1, 2, 3)) + (gd.abs() * amb).sum((1, 2, 3))
+    t1 = 2.0 ** -24 * chain * (gd * yf).abs().sum((1, 2, 3)) + ((gd * yf).abs() * amb).sum((1, 2, 3))
+    return s0, t0, s1, t1
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(n for n, c in CONV_CASES.items() if c["bwdstats"]))
 def test_conv_bwdstats_exact(be, name):
@@ -536,24 +586,8 @@ def test_conv_bwdstats_exact(be, name):
     beta = (0.3 * torch.randn(co, generator=gen)).float()
     scale = ((torch.rand((n, co), generator=gen) > 0.2).float() / 0.8).float()
     groups, eps, vox = 8, 1e-5, math.prod(ys)
-    # A, B as load_coefs forms them: fp64 group mean / rstd, rounded to fp32
-    cpg = co // groups
-    st = stats.view(n, groups, cpg, 2).sum(2)
-    m_ = float(cpg * vox)
-    mean = st[..., 0] / m_
-    var = (st[..., 1] / m_ - mean * mean).clamp_min(0)
-    rstd = 1.0 / torch.sqrt(var + eps)
-    mean_c, rstd_c = mean.repeat_interleave(cpg, 1), rstd.repeat_interleave(cpg, 1)
-    A = (rstd_c * gamma.double() * scale.double()).float().double().view(n, 1, 1, 1, co)
-    B = ((beta.double() - mean_c * rstd_c * gamma.double()) * scale.double()).float().double().view(n, 1, 1, 1, co)
-    z = yf * A + B
-    amb = z.abs() <= 2.0 ** -20 * ((yf * A).abs() + B.abs())
-    m = (z > 0).double()
-    gd = g_bf.double()
     chain = stats_chain(cs["path"], n, ys, co)
-    s0, s1 = (gd * m).sum((1, 2, 3)), (gd * m * yf).sum((1, 2, 3))
-    t0 = 2.0 ** -24 * chain * gd.abs().sum((1, 2, 3)) + (gd.abs() * amb).sum((1, 2, 3))
-    t1 = 2.0 ** -24 * chain * (gd * yf).abs().sum((1, 2, 3)) + ((gd * yf).abs() * amb).sum((1, 2, 3))
+    s0, t0, s1, t1 = bwdstats_want(g_bf, yf, stats, gamma, beta, scale, groups, eps, chain)
 
     gx = Guarded((n,) + xs + (ci,), torch.bfloat16, fill=IN_FILL, device="cuda")
     gx.view.copy_(x.bfloat16())

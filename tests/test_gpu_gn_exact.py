@@ -1155,6 +1155,17 @@ def pool_input(dims, n, sp, c, gen, device="cuda"):
     return x.double(), w
 
 
+def pool_ref(dims, x, go):
+    """torch.max_pool3d (2 x 2 [x 2]) of x (N,D,H,W,C) float64 and its autograd for the output gradient go ->
+    (pooled, gradient w.r.t. x), both (N,D,H,W,C)"""
+    k = (2, 2, 2) if dims == 3 else (1, 2, 2)
+    xq = _ncdhw(x).contiguous().requires_grad_(True)
+    with torch.enable_grad():
+        o = F.max_pool3d(xq, k, k)
+        o.backward(_ncdhw(go).contiguous())
+    return _ndhwc(o.detach()), _ndhwc(xq.grad)
+
+
 def test_pool_input_has_every_tie_count():
     for dims in (3, 2):
         sp = (8, 8, 8) if dims == 3 else (1, 16, 16)
@@ -1175,11 +1186,7 @@ def test_pool_exact(be, name):
     osp = (sp[0] // k[0], sp[1] // 2, sp[2] // 2)
     go = torch.randint(-8, 9, (n,) + osp + (c,), generator=gen, device="cuda").double() / 8
     add = torch.randint(-8, 9, (n,) + sp + (c,), generator=gen, device="cuda").double() / 16
-    xq = _ncdhw(x).contiguous().requires_grad_(True)
-    with torch.enable_grad():
-        o = F.max_pool3d(xq, k, k)
-        o.backward(_ncdhw(go).contiguous())
-    want_o, want_g = _ndhwc(o.detach()), _ndhwc(xq.grad)
+    want_o, want_g = pool_ref(dims, x, go)
     gx, ggo, gad = _input(x, dt, off), _input(go, dt, off), _input(add, dt, off)
     out = pitched((n,) + osp + (c,), dt, off=off)
     be.pool_fwd(gx.view, out.view, dims)
