@@ -635,6 +635,47 @@ int b200seg_augment3d(const float* x, const void* y, int y_dtype, int n, int D, 
                       int rescale_mode, float* x_out, void* y_out, int label_out, int binarize, void* ws,
                       int64_t ws_bytes, int device, b200seg_stream stream);
 
+/* ---- mask post-processing (dataprocess/utils.py:7-66; SimpleITK on the CPU there).  One dense mask of (D, H, W)
+ * voxels, a 2-D mask as D = 1, D * H * W < 2^31; mask dtypes B200SEG_U8 (bool, uint8), B200SEG_I16, B200SEG_I32,
+ * B200SEG_I64, and for the morphology B200SEG_F32 too (NaN is nonzero).  Every result is an integer: reruns are
+ * bit-identical.
+ *
+ * b200seg_largest_component replaces GetLargestConnectedCompont (utils.py:19-44: sitk.ConnectedComponent with its
+ * default face connectivity, LabelIntensityStatisticsImageFilter and the loop over GetPhysicalSize): union-find
+ * labelling of the nonzero voxels over 6 (D > 1) or 4 face neighbours, each component labelled by its first voxel in
+ * C order.  out: uint8 [D][H][W], 1 on the component with the most voxels (ties: the earlier first voxel, ITK's
+ * raster-order labels) and 0 elsewhere, all 0 without foreground.  stats: int64 [2] = {number of components, voxels
+ * of the largest}.  Workspace: b200seg_components_workspace(D, H, W) bytes (8 per voxel).
+ *
+ * b200seg_morphology replaces MorphologicalOperation (utils.py:47-66: BinaryMorphologicalOpening / Closing,
+ * BinaryDilate, BinaryErode of mask != 0 with the default sitkBall of radius r).  The ball is {d : |d|^2 <= r^2 + r}
+ * over `dims` axes (ITK's FlatStructuringElement::Ball with axes 2r + 1).  DILATE: outside the image is background;
+ * ERODE: outside is foreground (BoundaryToForeground); OPEN: erode, then dilate; CLOSE: on the image padded by r on
+ * each of the `dims` axes with background (SafeBorder), dilate, erode, crop.  dims 2 needs D == 1; dims 3 with D == 1
+ * is a one-slice 3-D image.  out: uint8 0/1 [D][H][W].  0 <= radius <= B200SEG_MORPH_MAX_RADIUS; for CLOSE the
+ * padded grid must stay below 2^31 voxels.  Workspace: b200seg_morphology_workspace(...) bytes (4 per voxel of the
+ * grid, 5 for OPEN and CLOSE).
+ *
+ * b200seg_label_bbox replaces GetLargestConnectedCompontBoundingbox (utils.py:7-16:
+ * LabelShapeStatisticsImageFilter.GetBoundingBox(1) of the input itself, not of its largest component).  box: int64
+ * [2 dims + 1] = {x0, y0, [z0,] size x, size y, [size z,] voxels equal to 1}, all zero when no voxel equals 1 (ITK
+ * raises there).  Workspace: b200seg_label_bbox_workspace() bytes. */
+#define B200SEG_MORPH_DILATE 0
+#define B200SEG_MORPH_ERODE 1
+#define B200SEG_MORPH_OPEN 2
+#define B200SEG_MORPH_CLOSE 3
+#define B200SEG_MORPH_MAX_RADIUS 64
+int64_t b200seg_components_workspace(int D, int H, int W);
+int b200seg_largest_component(const void* mask, int mask_dtype, int D, int H, int W, void* workspace,
+                              int64_t workspace_bytes, uint8_t* out, int64_t* stats, int device,
+                              b200seg_stream stream);
+int64_t b200seg_morphology_workspace(int dims, int D, int H, int W, int radius, int op);
+int b200seg_morphology(const void* mask, int mask_dtype, int dims, int D, int H, int W, int radius, int op,
+                       void* workspace, int64_t workspace_bytes, uint8_t* out, int device, b200seg_stream stream);
+int64_t b200seg_label_bbox_workspace(void);
+int b200seg_label_bbox(const void* mask, int mask_dtype, int dims, int D, int H, int W, void* workspace,
+                       int64_t workspace_bytes, int64_t* box, int device, b200seg_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,9 @@ module raises as shipped, so its evident intent runs here, with four documented 
 ``inference_patch3d``), and the 2-D ``XModel.inference`` and datasets' bit-exact cv2 bilinear resize (``inference2d``,
 ``resize2d``, ``InputStager(max_source_pixels=...)``), and the 3-D data augmentation of
 ``dataprocess/Augmentation`` (``ImageDataGenerator3D``: scipy's order-0 affine warp bit for bit, offline through
-``DataAug3D`` or per training step through ``transform_batch``).
+``DataAug3D`` or per training step through ``transform_batch``), and the mask post-processing of ``dataprocess/utils.py``
+(``largest_component``, ``binary_morphology``, ``label_bbox`` and the reference-named ``GetLargestConnectedCompont``,
+``MorphologicalOperation``, ``GetLargestConnectedCompontBoundingbox``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -35,6 +37,8 @@ from .staging import InputStager, stage_batch
 from .ssim import SSIM, SSIM3D, ssim, ssim3D
 from .augment import ImageDataGenerator3D
 from .cldice import soft_skeletonize, norm_intersection, Binary_Soft_cldice_loss, Mutil_Soft_cldice_loss
+from .postprocess import (largest_component, binary_morphology, label_bbox, GetLargestConnectedCompont,
+                          MorphologicalOperation, GetLargestConnectedCompontBoundingbox)
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
@@ -45,4 +49,6 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "BinaryDiceFocalLoss", "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss",
            "MutilCrossEntropyDiceLoss", "BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "BinaryTverskyLoss",
            "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge", "SSIM", "SSIM3D", "ssim", "ssim3D",
-           "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss"]
+           "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss",
+           "largest_component", "binary_morphology", "label_bbox", "GetLargestConnectedCompont",
+           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox"]

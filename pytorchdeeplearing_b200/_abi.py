@@ -20,6 +20,9 @@ I64 = 16
 U8, I32 = 17, 18          # mask dtypes of the segmentation metrics
 I16 = 19                  # volumes of the whole-volume resample
 NORM_NONE, NORM_MEANSTD, NORM_PCTL = 0, 1, 2
+# operations of b200seg_morphology (B200SEG_MORPH_*) and its largest radius
+MORPH_OPS = {"dilate": 0, "erode": 1, "open": 2, "close": 3}
+MORPH_MAX_RADIUS = 64
 # kernel families of b200seg_conv / b200seg_wgrad (include/b200seg.h: B200SEG_CONV_*, B200SEG_WGRAD_*)
 CONV_PATHS = ("PW_MMA", "TC", "HALO2D", "HALO3", "HALO_WS", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
 WGRAD_PATHS = ("HALO_MMA", "TC", "STEM_MMA", "STEM", "SMALLCIN", "GENERIC")
@@ -152,6 +155,12 @@ _SIGNATURES = {
     "b200seg_augment3d_workspace": ([_i, _i, _i, _i], C.c_int64),
     "b200seg_augment3d": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, C.c_double, _i, C.c_double, _i, _vp, _vp, _i, _i,
                            _vp, _i64, _i, _vp], C.c_int),
+    "b200seg_components_workspace": ([_i, _i, _i], C.c_int64),
+    "b200seg_largest_component": ([_vp, _i, _i, _i, _i, _vp, _i64, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_morphology_workspace": ([_i, _i, _i, _i, _i, _i], C.c_int64),
+    "b200seg_morphology": ([_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
+    "b200seg_label_bbox_workspace": ([], C.c_int64),
+    "b200seg_label_bbox": ([_vp, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -1115,6 +1124,51 @@ class CudaBackend:
                                                rescale_mode, x_out.data_ptr(), y_out.data_ptr(), codes[y_out.dtype],
                                                1 if binarize else 0, _p(ws), 0 if ws is None else ws.numel(), dev,
                                                st))
+
+    # ------------------------------------------------------------------ mask post-processing (csrc/postprocess.cu)
+    _PP_DTYPES = {torch.bool: U8, torch.uint8: U8, torch.int16: I16, torch.int32: I32, torch.int64: I64,
+                  torch.float32: F32}
+
+    def _pp_mask(self, mask, allow_f32=False):
+        """dense (H, W) or (D, H, W) mask -> (dtype code, dims, D, H, W)"""
+        code = self._PP_DTYPES.get(mask.dtype)
+        if code is None or (code == F32 and not allow_f32):
+            raise TypeError(f"unsupported mask dtype {mask.dtype}")
+        assert mask.dim() in (2, 3) and mask.is_contiguous()
+        dims = mask.dim()
+        return (code, dims) + ((1,) + tuple(mask.shape) if dims == 2 else tuple(mask.shape))
+
+    def largest_component(self, mask, out, stats):
+        """out uint8 like mask: 1 on the face-connected component with the most voxels (ties: first in C order);
+        stats int64 [2] = {components, voxels of the largest}"""
+        dev, st = self._ds(mask)
+        code, _, d, h, w = self._pp_mask(mask)
+        assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == mask.numel()
+        assert stats.dtype == torch.int64 and stats.numel() >= 2
+        nb = int(self.lib.b200seg_components_workspace(d, h, w))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=mask.device)
+        self._check(self.lib.b200seg_largest_component(mask.data_ptr(), code, d, h, w, ws.data_ptr(), nb,
+                                                       out.data_ptr(), stats.data_ptr(), dev, st))
+
+    def morphology(self, mask, radius, op, out):
+        """op: MORPH_* code; out uint8 like mask (0/1)"""
+        dev, st = self._ds(mask)
+        code, dims, d, h, w = self._pp_mask(mask, allow_f32=True)
+        assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() == mask.numel()
+        nb = int(self.lib.b200seg_morphology_workspace(dims, d, h, w, radius, op))
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=mask.device)
+        self._check(self.lib.b200seg_morphology(mask.data_ptr(), code, dims, d, h, w, radius, op, ws.data_ptr(), nb,
+                                                out.data_ptr(), dev, st))
+
+    def label_bbox(self, mask, box):
+        """box int64 [2 dims + 1] = {x0, y0, [z0,] sx, sy, [sz,] voxels equal to 1}"""
+        dev, st = self._ds(mask)
+        code, dims, d, h, w = self._pp_mask(mask)
+        assert box.dtype == torch.int64 and box.numel() >= 2 * dims + 1
+        nb = int(self.lib.b200seg_label_bbox_workspace())
+        ws = torch.empty(nb, dtype=torch.uint8, device=mask.device)
+        self._check(self.lib.b200seg_label_bbox(mask.data_ptr(), code, dims, d, h, w, ws.data_ptr(), nb,
+                                                box.data_ptr(), dev, st))
 
     def mask_logits(self, logits, threshold, mask):
         dev, st = self._ds(logits)

@@ -202,6 +202,16 @@ long long augment3d_workspace(int n, long long vox);
 int augment3d(const float* x, const void* y, int y_dtype, int n, int D, int H, int W, int C,
               const b200seg_aug3d_param* params, int mode, double cval, int shift, double rescale, int rescale_mode,
               float* x_out, void* y_out, int label_out, int binarize, void* ws, cudaStream_t st);
+long long components_workspace(int D, int H, int W);
+int largest_component(const void* mask, int dt, int D, int H, int W, void* ws, unsigned char* out, long long* stats,
+                      int dev, cudaStream_t st);
+long long morphology_workspace(int dims, int D, int H, int W, int r, int op);
+long long morphology_voxels(int dims, int D, int H, int W, int r, int op);
+int morphology(const void* mask, int dt, int dims, int D, int H, int W, int r, int op, void* ws, unsigned char* out,
+               int dev, cudaStream_t st);
+long long label_bbox_workspace();
+int label_bbox(const void* mask, int dt, int dims, int D, int H, int W, void* ws, long long* box, int dev,
+               cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -1070,6 +1080,73 @@ int b200seg_augment3d(const float* x, const void* y, int y_dtype, int n, int D, 
   B200_DEVICE(device);
   return augment3d(x, y, y_dtype, n, D, H, W, C, params, fill_mode, cval, shift, rescale, rescale_mode, x_out, y_out,
                    label_out, binarize, ws, ST(stream));
+}
+
+// ---- mask post-processing (csrc/postprocess.cu)
+static bool valid_mask_dtype(int dt, bool allow_f32) {
+  return dt == B200SEG_U8 || dt == B200SEG_I16 || dt == B200SEG_I32 || dt == B200SEG_I64 ||
+         (allow_f32 && dt == B200SEG_F32);
+}
+
+static bool valid_mask_sizes(int dims, int D, int H, int W) {
+  return (dims == 3 || (dims == 2 && D == 1)) && D >= 1 && H >= 1 && W >= 1 && (long long)D * H * W < (1LL << 31);
+}
+
+static bool valid_morphology(int dims, int D, int H, int W, int radius, int op) {
+  return valid_mask_sizes(dims, D, H, W) && radius >= 0 && radius <= B200SEG_MORPH_MAX_RADIUS &&
+         op >= B200SEG_MORPH_DILATE && op <= B200SEG_MORPH_CLOSE &&
+         morphology_voxels(dims, D, H, W, radius, op) < (1LL << 31);
+}
+
+int64_t b200seg_components_workspace(int D, int H, int W) {
+  if (!valid_mask_sizes(3, D, H, W)) return 0;
+  return components_workspace(D, H, W);
+}
+
+int b200seg_largest_component(const void* mask, int mask_dtype, int D, int H, int W, void* workspace,
+                              int64_t workspace_bytes, uint8_t* out, int64_t* stats, int device,
+                              b200seg_stream stream) {
+  B200_CHECK_ARG(mask && workspace && out && stats, "b200seg_largest_component: null argument");
+  B200_CHECK_ARG(valid_mask_sizes(3, D, H, W), "b200seg_largest_component: bad sizes %d x %d x %d (D * H * W < 2^31)",
+                 D, H, W);
+  B200_CHECK_ARG(valid_mask_dtype(mask_dtype, false), "b200seg_largest_component: bad mask dtype %d", mask_dtype);
+  B200_CHECK_ARG(workspace_bytes >= b200seg_components_workspace(D, H, W),
+                 "b200seg_largest_component: workspace too small");
+  B200_DEVICE(device);
+  return largest_component(mask, mask_dtype, D, H, W, workspace, out, reinterpret_cast<long long*>(stats), device,
+                           ST(stream));
+}
+
+int64_t b200seg_morphology_workspace(int dims, int D, int H, int W, int radius, int op) {
+  if (!valid_morphology(dims, D, H, W, radius, op)) return 0;
+  return morphology_workspace(dims, D, H, W, radius, op);
+}
+
+int b200seg_morphology(const void* mask, int mask_dtype, int dims, int D, int H, int W, int radius, int op,
+                       void* workspace, int64_t workspace_bytes, uint8_t* out, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(mask && workspace && out, "b200seg_morphology: null argument");
+  B200_CHECK_ARG(mask != (const void*)out, "b200seg_morphology: out aliases the mask");
+  B200_CHECK_ARG(valid_morphology(dims, D, H, W, radius, op),
+                 "b200seg_morphology: bad arguments (dims %d, %d x %d x %d, radius %d, op %d; radius <= %d, the "
+                 "(padded) grid below 2^31 voxels)", dims, D, H, W, radius, op, B200SEG_MORPH_MAX_RADIUS);
+  B200_CHECK_ARG(valid_mask_dtype(mask_dtype, true), "b200seg_morphology: bad mask dtype %d", mask_dtype);
+  B200_CHECK_ARG(workspace_bytes >= b200seg_morphology_workspace(dims, D, H, W, radius, op),
+                 "b200seg_morphology: workspace too small");
+  B200_DEVICE(device);
+  return morphology(mask, mask_dtype, dims, D, H, W, radius, op, workspace, out, device, ST(stream));
+}
+
+int64_t b200seg_label_bbox_workspace(void) { return label_bbox_workspace(); }
+
+int b200seg_label_bbox(const void* mask, int mask_dtype, int dims, int D, int H, int W, void* workspace,
+                       int64_t workspace_bytes, int64_t* box, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(mask && workspace && box, "b200seg_label_bbox: null argument");
+  B200_CHECK_ARG(valid_mask_sizes(dims, D, H, W), "b200seg_label_bbox: bad sizes (dims %d, %d x %d x %d)", dims, D, H,
+                 W);
+  B200_CHECK_ARG(valid_mask_dtype(mask_dtype, false), "b200seg_label_bbox: bad mask dtype %d", mask_dtype);
+  B200_CHECK_ARG(workspace_bytes >= b200seg_label_bbox_workspace(), "b200seg_label_bbox: workspace too small");
+  B200_DEVICE(device);
+  return label_bbox(mask, mask_dtype, dims, D, H, W, workspace, reinterpret_cast<long long*>(box), device, ST(stream));
 }
 
 }  // extern "C"

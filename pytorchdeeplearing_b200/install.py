@@ -4,7 +4,8 @@ The reference wrappers bind the classes at import time (``from networks.VNet3d i
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
 rebinds those names in whichever of ``networks``, ``networks.*`` (``networks.Unet3dthin`` included), ``model.modelVNet``,
 ``model.modelUnet``, ``model.modelResNet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM``, ``model.lossescldice`` are already imported (and in ``sys.modules`` entries
-imported later via the same names).  ``ImageDataGenerator3D`` is rebound in ``dataprocess.Augmentation.
+imported later via the same names).  The mask post-processing functions are rebound in ``dataprocess.utils``.
+``ImageDataGenerator3D`` is rebound in ``dataprocess.Augmentation.
 images_masks_3dtransform`` and ``dataprocess.Augmentation.ImageAugmentation`` (which binds it at import,
 ImageAugmentation.py:1), so an unmodified ``DataAug3D(...).DataAugmentation(...)`` warps on the GPU.  ``uninstall``
 restores the originals.
@@ -26,11 +27,14 @@ _EXT_LOSS_NAMES = ("BinaryJaccardLoss", "BinaryELDiceLoss", "BinarySSLoss", "Bin
 _SSIM_NAMES = ("SSIM", "SSIM3D", "ssim", "ssim3D")
 # model/lossescldice.py
 _CLDICE_NAMES = ("soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss")
+# dataprocess/utils.py
+_POSTPROCESS_NAMES = ("GetLargestConnectedCompont", "GetLargestConnectedCompontBoundingbox", "MorphologicalOperation")
 _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d", "networks.Unet3dthin", "networks.Unet2d",
             "model",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
             "model.lossescldice", "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet",
-            "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation")
+            "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation",
+            "dataprocess.utils")
 
 
 def install() -> int:
@@ -38,12 +42,13 @@ def install() -> int:
     from . import networks as nets, losses, metric
     from .ssim import SSIM, SSIM3D, ssim, ssim3D       # the package's ``ssim`` attribute is the function, not the module
     from .augment import ImageDataGenerator3D
-    from . import cldice
+    from . import cldice, postprocess
     table = {n: getattr(nets, n) for n in _NET_NAMES}
     table.update({n: getattr(losses, n) for n in _LOSS_NAMES + _EXT_LOSS_NAMES})
     table.update({n: getattr(metric, n) for n in _METRIC_NAMES})     # per-step accuracy, model/modelVNet.py:582
     table.update(zip(_SSIM_NAMES, (SSIM, SSIM3D, ssim, ssim3D)))
     table.update({n: getattr(cldice, n) for n in _CLDICE_NAMES})
+    table.update({n: getattr(postprocess, n) for n in _POSTPROCESS_NAMES})
     table["ImageDataGenerator3D"] = ImageDataGenerator3D    # dataprocess/Augmentation (DataAug3D)
     count = 0
     for modname in _MODULES:
