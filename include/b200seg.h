@@ -676,6 +676,29 @@ int64_t b200seg_label_bbox_workspace(void);
 int b200seg_label_bbox(const void* mask, int mask_dtype, int dims, int D, int H, int W, void* workspace,
                        int64_t workspace_bytes, int64_t* box, int device, b200seg_stream stream);
 
+/* ---- Grad-CAM of ResNet2d (model/visualization.py:112-224, GradCAM; model/modelResNet.py:419-426,
+ * Grad_CAM_Visual).  One call per target stage, in forward order, then one final scale; the map is fp32 [N][H][W].
+ * act / grad: one stage's output and d(sum_i logit[i, t_i]) / d output, (N, 1, h, w, C), F32 or BF16, channel pitch,
+ * C <= 1024, N <= 65535.  Stage `layer` of `nlayers`:
+ *   w[n][c] = mean over the h*w pixels of grad (fp64 fixed-order sums), cam = max(sum_c w[c] act[..., c], 0),
+ *   s = (cam - min) / (1e-7 + (max - min)) per image in fp32, then OpenCV's INTER_LINEAR resize to (H, W) in fp32:
+ *   fx = (float)((d + 0.5) / (D / S) - 0.5), s0 = floor(fx), weights (1 - (fx - s0), fx - s0), clamped at the borders,
+ *   the horizontal pass first, every product rounded before the sum (a stage at (H, W) is copied).
+ *   out = s (layer 0) or out + s; the last stage divides by nlayers (np.mean over the stages).
+ * b200seg_gradcam_scale: out = (out - min) / (1e-7 + (max - min)) per image, in place.
+ * The workspace (b200seg_gradcam_workspace bytes, the largest over the stages of one map) carries the per-image min / max
+ * from the stage calls to the scale call.  Min and max go through atomics (exact, order-free), sums have a fixed
+ * order: reruns are bit-identical.  No allocation, no host synchronisation.
+ * b200seg_gradcam_target: dlogits [N][K] = one-hot of t_i (target >= 0: t_i = target; target < 0: the arg-max of
+ * logits row i, the first of equal maxima) and category [N] = t_i. */
+int64_t b200seg_gradcam_workspace(int n, int h, int w, int c);
+int b200seg_gradcam_layer(const b200seg_tensor* act, const b200seg_tensor* grad, int H, int W, int layer, int nlayers,
+                          void* workspace, int64_t workspace_bytes, float* out, int device, b200seg_stream stream);
+int b200seg_gradcam_scale(float* out, int n, int H, int W, void* workspace, int64_t workspace_bytes, int device,
+                          b200seg_stream stream);
+int b200seg_gradcam_target(const float* logits, int n, int k, int target, float* dlogits, int64_t* category,
+                           int device, b200seg_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

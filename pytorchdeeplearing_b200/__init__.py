@@ -13,7 +13,8 @@ module raises as shipped, so its evident intent runs here, with four documented 
 ``dataprocess/Augmentation`` (``ImageDataGenerator3D``: scipy's order-0 affine warp bit for bit, offline through
 ``DataAug3D`` or per training step through ``transform_batch``), and the mask post-processing of ``dataprocess/utils.py``
 (``largest_component``, ``binary_morphology``, ``label_bbox`` and the reference-named ``GetLargestConnectedCompont``,
-``MorphologicalOperation``, ``GetLargestConnectedCompontBoundingbox``).
+``MorphologicalOperation``, ``GetLargestConnectedCompontBoundingbox``), and Grad-CAM of ResNet2d
+(``grad_cam`` and the reference-named ``GradCAM`` of ``model/visualization.py``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -39,6 +40,7 @@ from .augment import ImageDataGenerator3D
 from .cldice import soft_skeletonize, norm_intersection, Binary_Soft_cldice_loss, Mutil_Soft_cldice_loss
 from .postprocess import (largest_component, binary_morphology, label_bbox, GetLargestConnectedCompont,
                           MorphologicalOperation, GetLargestConnectedCompontBoundingbox)
+from .gradcam import grad_cam, GradCAM
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
@@ -51,4 +53,4 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge", "SSIM", "SSIM3D", "ssim", "ssim3D",
            "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss",
            "largest_component", "binary_morphology", "label_bbox", "GetLargestConnectedCompont",
-           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox"]
+           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox", "grad_cam", "GradCAM"]

@@ -161,6 +161,10 @@ _SIGNATURES = {
     "b200seg_morphology": ([_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_label_bbox_workspace": ([], C.c_int64),
     "b200seg_label_bbox": ([_vp, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
+    "b200seg_gradcam_workspace": ([_i, _i, _i, _i], C.c_int64),
+    "b200seg_gradcam_layer": ([_PT, _PT, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
+    "b200seg_gradcam_scale": ([_vp, _i, _i, _i, _vp, _i64, _i, _vp], C.c_int),
+    "b200seg_gradcam_target": ([_vp, _i, _i, _i, _vp, _vp, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -1169,6 +1173,32 @@ class CudaBackend:
         ws = torch.empty(nb, dtype=torch.uint8, device=mask.device)
         self._check(self.lib.b200seg_label_bbox(mask.data_ptr(), code, dims, d, h, w, ws.data_ptr(), nb,
                                                 box.data_ptr(), dev, st))
+
+    # ------------------------------------------------------------------ Grad-CAM (csrc/gradcam.cu)
+    def gradcam_target(self, logits, target, dlogits, category):
+        """logits [N][K] fp32 -> dlogits [N][K] fp32 one-hot of each row's class and category [N] int64; target: a
+        class for every row, or -1 for the arg-max of each row"""
+        dev, st = self._ds(logits)
+        n, k = logits.shape
+        assert logits.is_contiguous() and dlogits.is_contiguous() and dlogits.shape == logits.shape
+        assert category.dtype == torch.int64 and category.numel() == n
+        self._check(self.lib.b200seg_gradcam_target(logits.data_ptr(), n, k, int(target), dlogits.data_ptr(),
+                                                    category.data_ptr(), dev, st))
+
+    def gradcam(self, stages, out):
+        """stages: [(act, grad)] in forward order, each (N, 1, h, w, C) channels-last; out: fp32 (N, H, W) contiguous,
+        the Grad-CAM map (per-stage scale and resize, mean over the stages, final scale)"""
+        dev, st = self._ds(out)
+        n, H, W = out.shape
+        assert out.dtype == torch.float32 and out.is_contiguous()
+        nb = max(int(self.lib.b200seg_gradcam_workspace(a.shape[0], a.shape[2], a.shape[3], a.shape[4]))
+                 for a, _ in stages)
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=out.device)
+        for i, (a, g) in enumerate(stages):
+            da, dg = _desc(a), _desc(g)
+            self._check(self.lib.b200seg_gradcam_layer(C.byref(da), C.byref(dg), H, W, i, len(stages), ws.data_ptr(),
+                                                       nb, out.data_ptr(), dev, st))
+        self._check(self.lib.b200seg_gradcam_scale(out.data_ptr(), n, H, W, ws.data_ptr(), nb, dev, st))
 
     def mask_logits(self, logits, threshold, mask):
         dev, st = self._ds(logits)

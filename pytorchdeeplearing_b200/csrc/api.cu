@@ -212,6 +212,12 @@ int morphology(const void* mask, int dt, int dims, int D, int H, int W, int r, i
 long long label_bbox_workspace();
 int label_bbox(const void* mask, int dt, int dims, int D, int H, int W, void* ws, long long* box, int dev,
                cudaStream_t st);
+long long gradcam_workspace(int n, int h, int w, int c);
+int gradcam_layer(const b200seg_tensor* act, const b200seg_tensor* grad, int H, int W, int layer, int nlayers,
+                  void* ws, float* out, cudaStream_t st);
+int gradcam_scale(float* out, int n, int H, int W, void* ws, cudaStream_t st);
+int gradcam_target(const float* logits, int n, int k, int target, float* dlogits, long long* category,
+                   cudaStream_t st);
 
 static bool valid_tensor(const b200seg_tensor* t) {
   return t && t->ptr && t->n > 0 && t->d > 0 && t->h > 0 && t->w > 0 && t->c > 0 && t->ld >= t->c &&
@@ -1147,6 +1153,53 @@ int b200seg_label_bbox(const void* mask, int mask_dtype, int dims, int D, int H,
   B200_CHECK_ARG(workspace_bytes >= b200seg_label_bbox_workspace(), "b200seg_label_bbox: workspace too small");
   B200_DEVICE(device);
   return label_bbox(mask, mask_dtype, dims, D, H, W, workspace, reinterpret_cast<long long*>(box), device, ST(stream));
+}
+
+// ---- Grad-CAM (csrc/gradcam.cu)
+static bool valid_cam_sizes(int n, int h, int w, int c) {
+  return n >= 1 && n <= 65535 && h >= 1 && w >= 1 && c >= 1 && c <= 1024 && (long long)h * w < (1LL << 31);
+}
+
+int64_t b200seg_gradcam_workspace(int n, int h, int w, int c) {
+  if (!valid_cam_sizes(n, h, w, c)) return 0;
+  return gradcam_workspace(n, h, w, c);
+}
+
+int b200seg_gradcam_layer(const b200seg_tensor* act, const b200seg_tensor* grad, int H, int W, int layer, int nlayers,
+                          void* workspace, int64_t workspace_bytes, float* out, int device, b200seg_stream stream) {
+  REQ_TENSOR(act, "act");
+  REQ_TENSOR(grad, "grad");
+  B200_CHECK_ARG(workspace && out, "b200seg_gradcam_layer: null argument");
+  B200_CHECK_ARG(same_geom(act, grad) && act->d == 1, "b200seg_gradcam_layer: act and grad must be (N, 1, h, w, C) of "
+                 "one shape");
+  B200_CHECK_ARG(valid_cam_sizes(act->n, act->h, act->w, act->c) && H >= 1 && W >= 1 && (long long)H * W < (1LL << 31),
+                 "b200seg_gradcam_layer: bad sizes (N %d, %d x %d, C %d -> %d x %d; N <= 65535, C <= 1024)", act->n,
+                 act->h, act->w, act->c, H, W);
+  B200_CHECK_ARG(nlayers >= 1 && layer >= 0 && layer < nlayers, "b200seg_gradcam_layer: bad layer %d of %d", layer,
+                 nlayers);
+  B200_CHECK_ARG(workspace_bytes >= b200seg_gradcam_workspace(act->n, act->h, act->w, act->c),
+                 "b200seg_gradcam_layer: workspace too small");
+  B200_DEVICE(device);
+  return gradcam_layer(act, grad, H, W, layer, nlayers, workspace, out, ST(stream));
+}
+
+int b200seg_gradcam_scale(float* out, int n, int H, int W, void* workspace, int64_t workspace_bytes, int device,
+                          b200seg_stream stream) {
+  B200_CHECK_ARG(workspace && out, "b200seg_gradcam_scale: null argument");
+  B200_CHECK_ARG(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && (long long)H * W < (1LL << 31),
+                 "b200seg_gradcam_scale: bad sizes (N %d, %d x %d)", n, H, W);
+  B200_CHECK_ARG(workspace_bytes >= 16LL * n, "b200seg_gradcam_scale: workspace too small");
+  B200_DEVICE(device);
+  return gradcam_scale(out, n, H, W, workspace, ST(stream));
+}
+
+int b200seg_gradcam_target(const float* logits, int n, int k, int target, float* dlogits, int64_t* category,
+                           int device, b200seg_stream stream) {
+  B200_CHECK_ARG(logits && dlogits && category, "b200seg_gradcam_target: null argument");
+  B200_CHECK_ARG(n >= 1 && k >= 1 && target < k, "b200seg_gradcam_target: bad arguments (N %d, K %d, target %d)", n, k,
+                 target);
+  B200_DEVICE(device);
+  return gradcam_target(logits, n, k, target, dlogits, reinterpret_cast<long long*>(category), ST(stream));
 }
 
 }  // extern "C"

@@ -33,6 +33,8 @@ K3, K1, DOWN, UP = 0, 1, 2, 3
 GROUPS = 8
 GN_EPS = 1e-5
 P_DROP = 0.2
+# the ResNet stages whose outputs Grad-CAM can take (resnet_backward ``stages``), in forward order
+RESNET_STAGES = ("in_tr", "down_tr32", "down_tr64", "down_tr128", "down_tr256")
 
 
 @dataclass
@@ -158,6 +160,7 @@ class Engine:
         self._pre_bwd = None                   # (flat, z64 buffer, z32 buffer) zeroed during forward for backward
         self._deferred = None                  # (side, fork event, pack plan, zero buffers) not launched yet
         self._ov = 0                           # scheduling options of this pass (overlap_mask), fixed at forward
+        self._data_only = False                # backward computes data gradients only (no weight-gradient convolutions)
 
     # ---------------------------------------------------------------- allocation helpers
     def new(self, like: Tensor, sp: Sequence[int], c: int, dtype=None) -> Tensor:
@@ -544,27 +547,8 @@ class Engine:
             if L.bname is not None:
                 be.colsum(dy, self._grad_view(L.bname))
         w = self.P[L.wname]
-        taps = _taps(L.kind, self.dims)
-        cin = L.x.shape[-1]
-        if L.kind == UP:
-            dwp = self.zeros((taps, cout, cin), torch.float32, dev)
-            wg = (DOWN, self.dims, dy, L.x, dwp)             # a = fine side (dy), b = coarse side (x)
-        else:
-            dwp = self.zeros((taps, cin, cout), torch.float32, dev)
-            wg = (L.kind, self.dims, L.x, dy, dwp)
-        # without a data gradient there is nothing to overlap with, unless the caller has more work for the main
-        # stream (``side_wgrad``: the other branch of the input block)
-        side = _side_stream(dev) if (need_dx or side_wgrad) else None
-        if side is not None:
-            # dW only feeds the final unpack: run it beside the dgrad -> next-layer chain
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):
-                be.wgrad(*wg)
-            self._side = side
-            self._side_keep.append(wg)
-        else:
-            be.wgrad(*wg)
-        self._unpack_list.append((dwp, self._grad_view(L.wname)))
+        if not self._data_only:
+            self._wgrad(L, dy, side=need_dx or side_wgrad)
         if not need_dx:
             return None
         wd = self._packs.get((L.wname, "dgrad"))
@@ -583,6 +567,31 @@ class Engine:
         else:
             be.conv(dkind, self.dims, dy, wd, None, dx_out, None, dx_addend)
         return dx_out
+
+    def _wgrad(self, L: Layer, dy: Tensor, side: bool) -> None:
+        """the weight gradient of ``bwd_layer``, queued for the final unpack"""
+        be, dev = self.be, dy.device
+        taps = _taps(L.kind, self.dims)
+        cin, cout = L.x.shape[-1], L.y.shape[-1]
+        if L.kind == UP:
+            dwp = self.zeros((taps, cout, cin), torch.float32, dev)
+            wg = (DOWN, self.dims, dy, L.x, dwp)             # a = fine side (dy), b = coarse side (x)
+        else:
+            dwp = self.zeros((taps, cin, cout), torch.float32, dev)
+            wg = (L.kind, self.dims, L.x, dy, dwp)
+        # without a data gradient there is nothing to overlap with, unless the caller has more work for the main
+        # stream (``side_wgrad``: the other branch of the input block)
+        st = _side_stream(dev) if side else None
+        if st is not None:
+            # dW only feeds the final unpack: run it beside the dgrad -> next-layer chain
+            st.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(st):
+                be.wgrad(*wg)
+            self._side = st
+            self._side_keep.append(wg)
+        else:
+            be.wgrad(*wg)
+        self._unpack_list.append((dwp, self._grad_view(L.wname)))
 
     def alloc_grads(self, device) -> Tensor:
         """One flat fp32 bucket; ``self.grads`` are views in state_dict order (the bucket is
@@ -825,11 +834,18 @@ class Engine:
         sv["head"] = (out, pooled, hidden)
         return logits
 
-    def resnet_backward(self, g_logits: Tensor) -> Tensor:
+    def resnet_backward(self, g_logits: Tensor, stages: Optional[Sequence[str]] = None):
         """Gradients of all 70 parameters given d loss / d logits ((N, numclass) fp32, contiguous).  Returns the flat
-        fp32 bucket; ``self.grads`` holds the views."""
+        fp32 bucket; ``self.grads`` holds the views.
+
+        ``stages`` (Grad-CAM): names from ``RESNET_STAGES``.  Then only data gradients are computed -- no weight-gradient
+        convolution runs, the GroupNorm, bias and head parameter gradients land in a scratch bucket -- and the pass stops
+        after the earliest stage asked for.  Returns {stage: (output, d loss / d output)}, channels-last in the engine's
+        dtype; the output of ``in_tr`` is the input of ``down_tr32.down_conv``, that of ``down_tr256`` the head input."""
         sv = self.saved
         dev = g_logits.device
+        want = set(stages or ())
+        self._data_only = stages is not None
         flat = self.alloc_grads(dev)
         n = g_logits.shape[0]
         self._begin_pass(n, dev, backward=True)
@@ -841,25 +857,36 @@ class Engine:
         gv = self._grad_view
         self.be.cls_head_bwd(g_logits, pooled, hidden, w1, w2, work, g, gv("fc_layers.0.weight"),
                              gv("fc_layers.0.bias"), gv("fc_layers.2.weight"), gv("fc_layers.2.bias"))
+        found = {}
         for i, name in zip((3, 2, 1, 0), ["down_tr256", "down_tr128", "down_tr64", "down_tr32"]):
             Ld, ops = sv[name]
+            if name in want:
+                found[name] = (out, g)
+                if len(found) == len(want):
+                    break
             g_out = g                                    # d/d(out) ; out = ops(down) + down
             gh = g_out
             for j in reversed(range(len(ops))):
                 gh = self.bwd_layer(ops[j], gh, True, dx_addend=g_out if j == 0 else None,
                                     prev=ops[j - 1] if j > 0 else Ld)
             g = self.bwd_layer(Ld, gh, True)
-            if i == 3:
+            out = Ld.x                                   # the previous stage's output
+            if i == 3 and not self._data_only:
                 self._flush_bucket("down_tr256.down_conv.weight")
                 self._early_unpack()
-        La, Lb = sv["in_tr"]
-        if La.wpk is not None:
-            self.stem_block_backward(La, Lb, g)
         else:
-            self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
-            self.bwd_layer(Lb, g, False)
+            if "in_tr" in want:
+                found["in_tr"] = (out, g)
+            elif not self._data_only:
+                La, Lb = sv["in_tr"]
+                if La.wpk is not None:
+                    self.stem_block_backward(La, Lb, g)
+                else:
+                    self.bwd_layer(La, g, False, side_wgrad=bool(self._ov & OV_TAIL))
+                    self.bwd_layer(Lb, g, False)
         self._finish_backward()
-        return flat
+        self._data_only = False
+        return found if stages is not None else flat
 
     # ================================================================== UNet3d / UNet2d
     def unet_forward(self, P: Dict[str, Tensor], x: Tensor, masks: Optional[List[Tensor]],

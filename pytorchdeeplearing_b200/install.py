@@ -4,7 +4,8 @@ The reference wrappers bind the classes at import time (``from networks.VNet3d i
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
 rebinds those names in whichever of ``networks``, ``networks.*`` (``networks.Unet3dthin`` included), ``model.modelVNet``,
 ``model.modelUnet``, ``model.modelResNet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM``, ``model.lossescldice`` are already imported (and in ``sys.modules`` entries
-imported later via the same names).  The mask post-processing functions are rebound in ``dataprocess.utils``.
+imported later via the same names).  The mask post-processing functions are rebound in ``dataprocess.utils``, and
+``GradCAM`` in ``model.visualization`` and ``model.modelResNet`` (so ``Grad_CAM_Visual`` runs on the GPU).
 ``ImageDataGenerator3D`` is rebound in ``dataprocess.Augmentation.
 images_masks_3dtransform`` and ``dataprocess.Augmentation.ImageAugmentation`` (which binds it at import,
 ImageAugmentation.py:1), so an unmodified ``DataAug3D(...).DataAugmentation(...)`` warps on the GPU.  ``uninstall``
@@ -34,7 +35,7 @@ _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
             "model.lossescldice", "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet",
             "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation",
-            "dataprocess.utils")
+            "dataprocess.utils", "model.visualization")
 
 
 def install() -> int:
@@ -43,6 +44,7 @@ def install() -> int:
     from .ssim import SSIM, SSIM3D, ssim, ssim3D       # the package's ``ssim`` attribute is the function, not the module
     from .augment import ImageDataGenerator3D
     from . import cldice, postprocess
+    from .gradcam import GradCAM
     table = {n: getattr(nets, n) for n in _NET_NAMES}
     table.update({n: getattr(losses, n) for n in _LOSS_NAMES + _EXT_LOSS_NAMES})
     table.update({n: getattr(metric, n) for n in _METRIC_NAMES})     # per-step accuracy, model/modelVNet.py:582
@@ -50,6 +52,7 @@ def install() -> int:
     table.update({n: getattr(cldice, n) for n in _CLDICE_NAMES})
     table.update({n: getattr(postprocess, n) for n in _POSTPROCESS_NAMES})
     table["ImageDataGenerator3D"] = ImageDataGenerator3D    # dataprocess/Augmentation (DataAug3D)
+    table["GradCAM"] = GradCAM                              # model/visualization.py, model/modelResNet.py
     count = 0
     for modname in _MODULES:
         mod = sys.modules.get(modname)
