@@ -260,6 +260,37 @@ class EmuBackend:
     def colsum(self, dy, out):
         out += dy.double().sum((0, 1, 2, 3)).float()
 
+    # ------------------------------------------------------------------ trilinear 2x upsample + skip add (UNet3dthin)
+    def upsample_add(self, a, e, s):
+        up = F.interpolate(_ncdhw(a), scale_factor=(2, 2, 2), mode="trilinear")
+        _store(s, up + _ncdhw(e))
+
+    def upsample_bwd(self, g_s, g_a):
+        with torch.enable_grad():
+            a = torch.zeros(_ncdhw(g_a).shape, requires_grad=True)
+            up = F.interpolate(a, scale_factor=(2, 2, 2), mode="trilinear")
+            (ga,) = torch.autograd.grad(up, a, _ncdhw(g_s))
+        _store(g_a, ga)
+
+    # ------------------------------------------------------------------ classifier head (ResNet2d / ResNet3d)
+    def cls_head_fwd(self, x, w1, b1, w2, b2, pooled, hidden, logits):
+        p = x.float().reshape(x.shape[0], -1, x.shape[-1]).mean(1)
+        h = F.relu(F.linear(p, w1, b1))
+        pooled.copy_(p)
+        hidden.copy_(h)
+        logits.copy_(F.linear(h, w2, b2))
+
+    def cls_head_bwd(self, dlogits, pooled, hidden, w1, w2, work, dx, dw1, db1, dw2, db2):
+        n, c = pooled.shape
+        vox = dx.numel() // (n * c)
+        dh = (dlogits @ w2) * (hidden > 0)
+        dp = (dh @ w1) / vox
+        dw1.copy_(dh.t() @ pooled)
+        db1.copy_(dh.sum(0))
+        dw2.copy_(dlogits.t() @ hidden)
+        db2.copy_(dlogits.sum(0))
+        dx.copy_(dp.view(n, 1, 1, 1, c).expand(dx.shape).to(dx.dtype))
+
     # ------------------------------------------------------------------ head + losses
     def head_probs(self, logits, probs):
         if logits.shape[-1] == 1:

@@ -52,6 +52,12 @@ from test_gpu_gn_exact import per_channel, ulp32, GROUPS, EPS, U
 BF, F32 = torch.bfloat16, torch.float32
 C = 16                        # output channels of both fused families
 CI = 32                       # up_tr32's input channels
+# the (channel pitch, channel offset) layouts the exact tests run the fused kernels' outputs and upstream gradients at.
+# They include the networks' own: VNet3d's input block writes the skip half of a 32-channel concat and ResNet3d's a
+# contiguous buffer; its g arrives contiguous from the next layer's data gradient; up_tr32 writes the left half of its
+# concat, reads the left half of the concat gradient and writes a contiguous dx.  (CI + 16, None): the case's dx_off.
+LAYOUTS = {"stem_gn out": ((C + 16, 16), (C, 0)), "stem_gn g": ((C + 16, 0), (C, 0)),
+           "up_gn out": ((C + 16, 0),), "up_gn g": ((C + 16, 0),), "up_gn dx": ((CI + 16, None), (CI, 0))}
 SM_TH = 8                     # stem tile rows (stem_mma.cuh:10)
 PW_TILE, UB_TILE = 512, 128   # up_gn tiles (pw_mma.cuh:11, up_gn.cu:33)
 EINVAL = -1                   # B200SEG_EINVAL (include/b200seg.h)
@@ -626,6 +632,13 @@ def _gn(b, vox, stats=None, eps=EPS):
             b["scale"].float().cuda(), vox, GROUPS, eps)
 
 
+def _at(c, layout, off=None):
+    """Guarded's arguments for a (pitch, offset) layout of c channels"""
+    ld, o = layout
+    assert ld in (c, c + 16)
+    return dict(dense=True) if ld == c else dict(off=off if o is None else o)
+
+
 def _f(t):
     return None if t is None else t.float().cuda()
 
@@ -681,15 +694,23 @@ def test_stem_gn_exact(be, name):
         for (_, got), raw, k in zip(sbuf, (d["ya_raw"], d["yb_raw"]), ("3x3x3", "1x1x1")):
             check_stats(got.cpu(), raw.cpu(), chain, f"{name} stats {k} (full mantissas)")
 
-    # APPLY into the right half of a 32-channel buffer
+    # APPLY into the right half of a 32-channel buffer, and into a contiguous one
     gna, gnb = _gn(d["br"][0], vox), _gn(d["br"][1], vox)
-    out = Guarded(shape, BF, device="cuda", off=16)
-    be.stem_gn_apply(gx.view, p3, b3, p1, b1, gna, gnb, out.view)
-    assert_bitwise(out.view, (d["sides"][0]["relu"] + d["sides"][1]["relu"]).float().bfloat16(), f"{name} apply")
-    assert_guards(out, f"{name} apply")
+    for lay in LAYOUTS["stem_gn out"]:
+        out = Guarded(shape, BF, device="cuda", **_at(C, lay))
+        be.stem_gn_apply(gx.view, p3, b3, p1, b1, gna, gnb, out.view)
+        assert_bitwise(out.view, (d["sides"][0]["relu"] + d["sides"][1]["relu"]).float().bfloat16(),
+                       f"{name} apply {lay}")
+        assert_guards(out, f"{name} apply {lay}")
+    for lay in LAYOUTS["stem_gn g"]:
+        _stem_backward(be, name, cs, d, inexact, n, sp, sms, walk, gx, p3, b3, p1, b1, gna, gnb, lay)
 
-    # BSUMS over the left half of a concat gradient whose right half holds IN_FILL
-    gg = Guarded(shape, BF, fill=IN_FILL, device="cuda", off=0)
+
+def _stem_backward(be, name, cs, d, inexact, n, sp, sms, walk, gx, p3, b3, p1, b1, gna, gnb, lay):
+    """BSUMS and BWD of one stem case with g at layout `lay` (a concat-gradient half: the other half holds IN_FILL)"""
+    shape = (n,) + sp + (C,)
+    name = f"{name} g {lay}"
+    gg = Guarded(shape, BF, fill=IN_FILL, device="cuda", **_at(C, lay))
     gg.view.copy_(d["g"].bfloat16())
     sums = [flat((n, C, 3), torch.float64) for _ in range(2)]
     be.stem_gn_bwd_sums(gx.view, p3, b3, p1, b1, gna, gnb, gg.view, sums[0][1], sums[1][1])
@@ -763,9 +784,15 @@ def test_up_gn_exact(be, name):
     assert_equal64(s, d["side"]["sums"], f"{name} bwd sums")
     assert_flat_guards(sb, "sums")
 
+    for lay in LAYOUTS["up_gn dx"]:
+        _up_backward(be, f"{name} dx {lay}", cs, d, inexact, n, sp, sms, gx, wf, b, gn, gg, lay)
+
+
+def _up_backward(be, name, cs, d, inexact, n, sp, sms, gx, wf, b, gn, gg, lay):
+    """BWD of one up_tr32 case with dx at layout `lay`"""
     dwb, dw = flat((8, C, CI), F32, d["dw_pre"].float())
     pb = {k: flat((C,), F32, v.float()) for k, v in d["prefill"].items()}
-    gdx = Guarded((n,) + sp + (CI,), BF, device="cuda", off=cs["dx_off"])
+    gdx = Guarded((n,) + sp + (CI,), BF, device="cuda", **_at(CI, lay, cs["dx_off"]))
     be.up_gn_bwd(gx.view, wf, b, gn, gg.view, d["sums"].cuda(), dw, gdx.view, pb["dgamma"][1], pb["dbeta"][1],
                  None if not cs["bias"] else pb["dbias"][1])
     torch.cuda.synchronize()

@@ -189,14 +189,17 @@ def per_channel(t, cpg):
     return t.repeat_interleave(cpg, -1)
 
 
-def gn_branch(gen, N, C, vox):
-    """gamma, beta, scale, per-group mean / rstd and the per-channel statistics of one exact GroupNorm layer"""
+def gn_branch(gen, N, C, vox, drop=True):
+    """gamma, beta, scale, per-group mean / rstd and the per-channel statistics of one exact GroupNorm layer; without
+    `drop` the scale is 1 everywhere (a layer without Dropout passes no scale)"""
     cpg = C // GROUPS
     mu = torch.randint(-1, 2, (N, GROUPS), generator=gen).double()
     rs = 2.0 ** torch.randint(0, 2, (N, GROUPS), generator=gen).double()
     gamma = torch.randint(2, 7, (C,), generator=gen).double() / 4 * (torch.randint(0, 2, (C,), generator=gen) * 2 - 1)
     beta = torch.randint(-8, 9, (C,), generator=gen).double() / 16
     scale = torch.where(torch.rand((N, C), generator=gen) < 0.2, 0.0, 1.25).double()
+    if not drop:
+        scale = torch.ones_like(scale)
     mu_c, rs_c = per_channel(mu, cpg), per_channel(rs, cpg)
     for _ in range(64):           # move beta until no alphabet y sits exactly on a threshold
         A = rs_c * gamma * scale
@@ -233,12 +236,12 @@ def param_contribs(b, sums, co, vox, s3):
     return dict(dbeta=s1, dgamma=rs * (s2 - mu * s1), dbias=rs * b["gamma"] * s1 + co["Q"] * s3 + co["R"] * vox)
 
 
-def design(cs, seed=0):
+def design(cs, seed=0, drop=True):
     """the exact operands of one case (small per-channel tensors; the big ones are drawn on the device)"""
     gen = torch.Generator().manual_seed(seed)
     N, C, vox = cs["n"], cs["c"], math.prod(cs["sp"])
     cpg, m = C // GROUPS, C // GROUPS * vox
-    b1, b2 = gn_branch(gen, N, C, vox), gn_branch(gen, N, C, vox)
+    b1, b2 = gn_branch(gen, N, C, vox, drop), gn_branch(gen, N, C, vox, drop)
     a = torch.randint(-1, 2, (N, C), generator=gen).double() / 16
     bb = torch.randint(-1, 2, (N, C), generator=gen).double() / 16
     for _ in range(64):           # nudge a until neither m2 nor R nearly cancels

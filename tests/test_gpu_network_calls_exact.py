@@ -37,7 +37,8 @@ OPS = ("conv", "conv_bwdstats", "wgrad", "pool_fwd", "pool_bwd")
 FAMILY = {"conv": "conv", "conv_bwdstats": "bwdstats", "wgrad": "wgrad", "pool_fwd": "pool", "pool_bwd": "pool"}
 BLOCK = 512                   # bytes: the alignment a rebuilt view keeps
 GUARD_BLOCKS = 2              # guard band before and after every rebuilt storage, in blocks
-DTYPES = {"bfloat16": torch.bfloat16, "float32": torch.float32}
+DTYPES = {"bfloat16": torch.bfloat16, "float32": torch.float32, "float64": torch.float64}
+FILL_BITS = {**OUT_BITS, torch.float64: (torch.int64, 0x7FF80000DEADBEEF)}     # NaN payloads of a fresh output
 
 # forward statistics that are not compared with fp64, by kernel family, with the reason.  Every family the networks
 # reach has a chain bound in stats_chain, so none is exempt; a family added to the library must be derived there or
@@ -88,19 +89,21 @@ class Recorder:
     set by Engine._tag to the block the next launches belong to.  On the emulated backend, whose packed operands are
     plain tensors, the pack calls are wrapped too so that each operand's kind, which and dims are known."""
 
-    def __init__(self, inner, names=None):
+    def __init__(self, inner, names=None, ops=OPS, hook=None):
         self.inner = inner
         self.tag = "other"
         self.calls = []
         self.names = names or {}              # data_ptr of a parameter -> its name (labels only)
+        self.ops = ops                        # the entry points recorded
+        self.hook = hook                      # (recorder, op, args, kwargs) -> record dict; default: _record
         self._packed = {}                     # emulated backend: id(packed tensor) -> (packed, src, kind, which, dims)
 
     def __getattr__(self, name):
         fn = getattr(self.inner, name)
-        if name in OPS:
-            def record(*a):
-                self.calls.append(self._record(name, a))
-                return fn(*a)
+        if name in self.ops:
+            def record(*a, **k):
+                self.calls.append(self._record(name, a) if self.hook is None else self.hook(self, name, a, k))
+                return fn(*a, **k)
             return record
         if name in ("pack_weight", "pack_many", "pack_plan") and not hasattr(self.inner, "conv_path"):
             def pack(*a, **k):
@@ -152,8 +155,9 @@ class Recorder:
         return {"sig": sig, "tag": self.tag, "weight": None if src is None else self.names.get(src.data_ptr())}
 
 
-def record_step(backend, workload, precision, device, table=WORKLOADS):
-    """one eager training step of the workload in train mode (dropout on) -> (recorded calls, parameter names)"""
+def record_step(backend, workload, precision, device, table=WORKLOADS, ops=OPS, hook=None):
+    """one eager training step of the workload in train mode (dropout on) -> (recorded calls, parameter names, model);
+    `ops` and `hook` go to Recorder"""
     import pytorchdeeplearing_b200 as b200
     from pytorchdeeplearing_b200 import runtime
     net, args, n, sp = table[workload]
@@ -172,7 +176,7 @@ def record_step(backend, workload, precision, device, table=WORKLOADS):
         y, loss = (torch.rand((n,) + sp, generator=g) > 0.7).long(), b200.BinaryDiceLoss()
     else:
         y, loss = torch.randint(0, ncls, (n,) + sp, generator=g), b200.MutilDiceLoss(torch.ones(ncls, device=device))
-    rec = Recorder(backend, {p.data_ptr(): name for name, p in m.named_parameters()})
+    rec = Recorder(backend, {p.data_ptr(): name for name, p in m.named_parameters()}, ops, hook)
     runtime._set_backend_for_testing(rec)
     try:
         out = m(x.to(device))
@@ -216,7 +220,7 @@ class Rebuilt:
         self.s0 = a0 + (gb + mis) // es                    # first element of the rebuilt storage
         self.guard = (a0 * es, gb + mis, gb)
         if fill is None:
-            ib, pat = OUT_BITS[self.dtype]
+            ib, pat = FILL_BITS[self.dtype]
             self.buf.view(ib).fill_(pat)
         else:
             self.buf.fill_(fill)
@@ -236,7 +240,7 @@ class Rebuilt:
     def changed(self, inside=False):
         """None, or a description of the first element whose bits changed since the snapshot (outside the view only,
         unless `inside`)"""
-        ib = OUT_BITS[self.dtype][0]
+        ib = FILL_BITS[self.dtype][0]
         ne = self.buf.view(ib) != self.before.view(ib)
         if not inside:
             ne.as_strided(self.r.sizes, self.r.strides, self.s0 + self.r.offset).fill_(False)
@@ -245,6 +249,8 @@ class Rebuilt:
         i = int(ne.nonzero()[0]) - self.s0
         if i < 0 or i >= self.r.storage:
             return f"element {i} of the storage, in the guard band"
+        if len(self.r.strides) != 5:
+            return f"element {i} of the storage, outside the view"
         ld, off = pitch(self.r)
         return (f"element {i} of the storage (row {i // ld}, channel {i % ld - off} of the view's pitch), in the "
                 f"{'storage' if inside else 'storage outside the view (other concat half or pitch gap)'}")

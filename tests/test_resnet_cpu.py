@@ -10,7 +10,6 @@ import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
-import torch.nn.functional as F
 
 import oracle
 from oracle import resnet as ores
@@ -30,25 +29,7 @@ LOSSES = ("MutilCrossEntropyLoss", "MutilFocalLoss", "BinaryCrossEntropyLoss", "
 
 
 class ClsEmuBackend(EmuBackend):
-    """EmuBackend plus the two classifier-head entry points (b200seg_cls_head_fwd / _bwd) in torch ops"""
-
-    def cls_head_fwd(self, x, w1, b1, w2, b2, pooled, hidden, logits):
-        p = x.float().reshape(x.shape[0], -1, x.shape[-1]).mean(1)
-        h = F.relu(F.linear(p, w1, b1))
-        pooled.copy_(p)
-        hidden.copy_(h)
-        logits.copy_(F.linear(h, w2, b2))
-
-    def cls_head_bwd(self, dlogits, pooled, hidden, w1, w2, work, dx, dw1, db1, dw2, db2):
-        n, c = pooled.shape
-        vox = dx.numel() // (n * c)
-        dh = (dlogits @ w2) * (hidden > 0)
-        dp = (dh @ w1) / vox
-        dw1.copy_(dh.t() @ pooled)
-        db1.copy_(dh.sum(0))
-        dw2.copy_(dlogits.t() @ hidden)
-        db2.copy_(dlogits.sum(0))
-        dx.copy_(dp.view(n, 1, 1, 1, c).expand(dx.shape).to(dx.dtype))
+    """the emulated backend; its classifier-head entry points (b200seg_cls_head_fwd / _bwd) are torch ops"""
 
 
 @pytest.fixture(autouse=True)

@@ -9,14 +9,13 @@ import numpy as np
 import pytest
 import torch
 import torch.multiprocessing as mp
-import torch.nn.functional as F
 
 import oracle
 from oracle import nets as onets
 from oracle import unetthin as othin
 import pytorchdeeplearing_b200 as b200
 from pytorchdeeplearing_b200 import runtime
-from emu_backend import EmuBackend, _ncdhw, _store
+from emu_backend import EmuBackend
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -34,18 +33,7 @@ CASES = {
 
 
 class ThinEmuBackend(EmuBackend):
-    """the emulated backend plus the two upsample ops (torch's trilinear interpolation and its autograd)"""
-
-    def upsample_add(self, a, e, s):
-        up = F.interpolate(_ncdhw(a), scale_factor=(2, 2, 2), mode="trilinear")
-        _store(s, up + _ncdhw(e))
-
-    def upsample_bwd(self, g_s, g_a):
-        with torch.enable_grad():
-            a = torch.zeros(_ncdhw(g_a).shape, requires_grad=True)
-            up = F.interpolate(a, scale_factor=(2, 2, 2), mode="trilinear")
-            (ga,) = torch.autograd.grad(up, a, _ncdhw(g_s))
-        _store(g_a, ga)
+    """the emulated backend; its two upsample ops are torch's trilinear interpolation and its autograd"""
 
 
 @pytest.fixture()
