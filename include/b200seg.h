@@ -635,6 +635,53 @@ int b200seg_augment3d(const float* x, const void* y, int y_dtype, int n, int D, 
                       int rescale_mode, float* x_out, void* y_out, int label_out, int binarize, void* ws,
                       int64_t ws_bytes, int device, b200seg_stream stream);
 
+/* ---- 2-D augmentation: Segmenation_Aug (dataprocess/AugData.py), albumentations' HorizontalFlip, VerticalFlip,
+ * OneOf(MotionBlur, MedianBlur, Blur), ShiftScaleRotate and RandomBrightnessContrast, byte for byte OpenCV 4.13's
+ * uint8 cv2.flip, cv2.filter2D, cv2.medianBlur(3), cv2.blur((3, 3)), cv2.warpAffine (INTER_LINEAR for images,
+ * INTER_NEAREST for masks, BORDER_REFLECT_101) and cv2.LUT.  One entry per image (device memory, n entries): its
+ * source at byte offset src of src, dense (h, w, c) rows with c in {1, 3} interleaved; its output at byte offset dst
+ * of out, same layout; optionally a (h, w) mask at mask_src of msrc (mask_src < 0: none) written at mask_dst of mout.
+ * Stages, in this order, each applied when its bit of flags is set:
+ *   HFLIP / VFLIP: image and mask;
+ *   BLUR: blur = MOTION: filter2D over the ntaps taps (tap_dy, tap_dx offsets from the centre, tap_w weights, in the
+ *     kernel's row-major order), reflect-101, fp32, s = fma(v, w, s) for the row elements x * filter_cn + ch below
+ *     (w * filter_cn) & ~3 and s + v * w (rounded separately) above, cvRound (OpenCV's AVX2 body and scalar tail;
+ *     filter_cn is the channel count of the row cv2 filtered, c itself or 3 for a gray image read back from the
+ *     reference's BGR files); MEDIAN: the 3x3 median, replicated border; BOX: rint(3x3 sum / 9), reflect-101;
+ *   WARP: minv the inverse 2x3 matrix (cv2.invertAffineTransform, fp64); OpenCV's fixed-point map
+ *     adelta = rint(minv[0] x 1024), X0 = rint((minv[1] y + minv[2]) 1024) + 16, X = (X0 + adelta) >> 5 (fp64
+ *     products and sums rounded one by one), tap x = X >> 5, fraction X & 31 (likewise y with minv[3..5]); taps
+ *     reflected (101); v = (sum of taps x 32 (32 - f)(32 - f') products + 2^14) >> 15.  The mask: (X0 + 512 +
+ *     adelta) >> 10, reflected;
+ *   LUT: v = lut[v] (image only).
+ * The blur writes the blurred image into ws at the entry's dst offset (ws_bytes >= out_bytes =
+ * b200seg_augment2d_workspace(out_bytes)); stages is the OR of every entry's flags: without BLUR the blur launch is
+ * skipped and ws may be null.  max_hw >= every entry's h * w.  h, w in [1, 8192], n <= 65535; outputs must not alias
+ * inputs.  No reductions: reruns are bit-identical. */
+#define B200SEG_AUG2D_HFLIP 1
+#define B200SEG_AUG2D_VFLIP 2
+#define B200SEG_AUG2D_BLUR 4
+#define B200SEG_AUG2D_WARP 8
+#define B200SEG_AUG2D_LUT 16
+#define B200SEG_AUG2D_MOTION 1
+#define B200SEG_AUG2D_MEDIAN 2
+#define B200SEG_AUG2D_BOX 3
+#define B200SEG_AUG2D_MAX_TAPS 8
+#define B200SEG_AUG2D_MAX_SIDE 8192
+typedef struct b200seg_aug2d_param {
+  int64_t src, dst;           /* byte offsets of the image in src and of its output in out (and ws) */
+  int64_t mask_src, mask_dst; /* byte offsets of the mask in msrc and mout; mask_src < 0: no mask */
+  double minv[6];             /* inverse warp matrix, row-major 2x3 */
+  float tap_w[8];             /* motion kernel weights of the nonzero taps */
+  int8_t tap_dy[8], tap_dx[8];
+  int32_t h, w, c, flags, blur, ntaps, filter_cn, pad;
+  uint8_t lut[256];
+} b200seg_aug2d_param; /* 416 bytes */
+int64_t b200seg_augment2d_workspace(int64_t out_bytes);
+int b200seg_augment2d(const uint8_t* src, const uint8_t* msrc, const b200seg_aug2d_param* params, int n,
+                      int64_t max_hw, int stages, uint8_t* out, int64_t out_bytes, uint8_t* mout, void* ws,
+                      int64_t ws_bytes, int device, b200seg_stream stream);
+
 /* ---- mask post-processing (dataprocess/utils.py:7-66; SimpleITK on the CPU there).  One dense mask of (D, H, W)
  * voxels, a 2-D mask as D = 1, D * H * W < 2^31; mask dtypes B200SEG_U8 (bool, uint8), B200SEG_I16, B200SEG_I32,
  * B200SEG_I64, and for the morphology B200SEG_F32 too (NaN is nonzero).  Every result is an integer: reruns are

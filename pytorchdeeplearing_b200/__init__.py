@@ -14,7 +14,9 @@ module raises as shipped, so its evident intent runs here, with four documented 
 ``DataAug3D`` or per training step through ``transform_batch``), and the mask post-processing of ``dataprocess/utils.py``
 (``largest_component``, ``binary_morphology``, ``label_bbox`` and the reference-named ``GetLargestConnectedCompont``,
 ``MorphologicalOperation``, ``GetLargestConnectedCompontBoundingbox``), and Grad-CAM of ResNet2d
-(``grad_cam`` and the reference-named ``GradCAM`` of ``model/visualization.py``).
+(``grad_cam`` and the reference-named ``GradCAM`` of ``model/visualization.py``), and the 2-D data augmentation of
+``dataprocess/AugData.py`` (``Segmenation_Aug``: cv2's flips, blurs, warp and table byte for byte, offline through
+``DataAugmentation`` or per training step through ``transform_batch`` and ``InputStager(augment=...)``).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -41,6 +43,7 @@ from .cldice import soft_skeletonize, norm_intersection, Binary_Soft_cldice_loss
 from .postprocess import (largest_component, binary_morphology, label_bbox, GetLargestConnectedCompont,
                           MorphologicalOperation, GetLargestConnectedCompontBoundingbox)
 from .gradcam import grad_cam, GradCAM
+from .augment2d import Segmenation_Aug
 
 __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
@@ -53,4 +56,4 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge", "SSIM", "SSIM3D", "ssim", "ssim3D",
            "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss",
            "largest_component", "binary_morphology", "label_bbox", "GetLargestConnectedCompont",
-           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox", "grad_cam", "GradCAM"]
+           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox", "grad_cam", "GradCAM", "Segmenation_Aug"]

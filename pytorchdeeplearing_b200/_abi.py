@@ -152,6 +152,8 @@ _SIGNATURES = {
     "b200seg_normalize": ([_i, _vp, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_resample_nearest_u8": ([_vp, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp], C.c_int),
     "b200seg_resize_linear_u8": ([_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp], C.c_int),
+    "b200seg_augment2d_workspace": ([_i64], C.c_int64),
+    "b200seg_augment2d": ([_vp, _vp, _vp, _i, _i64, _i, _vp, _i64, _vp, _vp, _i64, _i, _vp], C.c_int),
     "b200seg_augment3d_workspace": ([_i, _i, _i, _i], C.c_int64),
     "b200seg_augment3d": ([_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, C.c_double, _i, C.c_double, _i, _vp, _vp, _i, _i,
                            _vp, _i64, _i, _vp], C.c_int),
@@ -203,6 +205,32 @@ RESIZE_SRC_BYTES = 16      # sizeof(struct b200seg_resize_src)
 def resize_src_table(entries) -> bytes:
     """[(byte offset, h, w)] of a ragged uint8 batch -> the host bytes of its ``b200seg_resize_src`` table"""
     return b"".join(struct.pack("<qii", int(o), int(h), int(w)) for o, h, w in entries)
+
+
+# stage bits and blur kinds of b200seg_augment2d (B200SEG_AUG2D_*)
+AUG2D_HFLIP, AUG2D_VFLIP, AUG2D_BLUR, AUG2D_WARP, AUG2D_LUT = 1, 2, 4, 8, 16
+AUG2D_BLURS = {"motion": 1, "median": 2, "box": 3}
+AUG2D_MAX_TAPS = 8
+AUG2D_MAX_SIDE = 8192
+AUG2D_PARAM_BYTES = 416    # sizeof(struct b200seg_aug2d_param)
+
+
+def aug2d_param_entry(src, dst, mask_src, mask_dst, h, w, c, flags, blur=0, taps=(), minv=None, lut=None,
+                      filter_cn=None) -> bytes:
+    """one ``b200seg_aug2d_param``: byte offsets, size, stage bits, blur kind, motion taps [(dy, dx, weight)],
+    inverse 2x3 matrix (fp64) and the 256-byte table"""
+    taps = list(taps)
+    if len(taps) > AUG2D_MAX_TAPS:
+        raise ValueError(f"at most {AUG2D_MAX_TAPS} motion-kernel taps, got {len(taps)}")
+    wt = [float(t[2]) for t in taps] + [0.0] * (AUG2D_MAX_TAPS - len(taps))
+    dy = [int(t[0]) for t in taps] + [0] * (AUG2D_MAX_TAPS - len(taps))
+    dx = [int(t[1]) for t in taps] + [0] * (AUG2D_MAX_TAPS - len(taps))
+    m = [0.0] * 6 if minv is None else [float(v) for v in minv]
+    table = bytes(256) if lut is None else bytes(lut)
+    assert len(table) == 256
+    return struct.pack("<4q6d8f8b8b8i", int(src), int(dst), int(mask_src), int(mask_dst), *m, *wt, *dy, *dx,
+                       int(h), int(w), int(c), int(flags), int(blur), len(taps),
+                       int(c if filter_cn is None else filter_cn), 0) + table
 
 
 # fill modes and rescale forms of b200seg_augment3d (B200SEG_AUG_*, B200SEG_RESCALE_*)
@@ -1104,6 +1132,24 @@ class CudaBackend:
         n, oh, ow = out.shape
         self._check(self.lib.b200seg_resize_linear_u8(src.data_ptr(), desc.data_ptr(), n, oh, ow, out.data_ptr(), mode,
                                                       dev, st))
+
+    # ------------------------------------------------------------------ 2-D augmentation (csrc/augment2d.cu)
+    def augment2d_workspace(self, out_bytes, device):
+        """uint8 workspace of b200seg_augment2d_workspace bytes (the blurred images)"""
+        nb = int(self.lib.b200seg_augment2d_workspace(int(out_bytes)))
+        return torch.empty(max(nb, 16), dtype=torch.uint8, device=device)
+
+    def augment2d(self, src, params, n, max_hw, stages, out, msrc=None, mout=None, ws=None):
+        """Segmenation_Aug's stages on a ragged uint8 batch: src / msrc flat uint8 device buffers holding every
+        image / mask, params uint8 device bytes of n ``aug2d_param_entry`` entries, out / mout flat uint8 outputs,
+        ws a workspace of ``augment2d_workspace(out.numel())`` when ``stages`` has AUG2D_BLUR"""
+        dev, st = self._ds(src)
+        for t in (src, out, msrc, mout, ws, params):
+            assert t is None or (t.dtype == torch.uint8 and t.is_contiguous())
+        assert params.numel() >= n * AUG2D_PARAM_BYTES
+        self._check(self.lib.b200seg_augment2d(src.data_ptr(), _p(msrc), params.data_ptr(), int(n), int(max_hw),
+                                               int(stages), out.data_ptr(), out.numel(), _p(mout), _p(ws),
+                                               0 if ws is None else ws.numel(), dev, st))
 
     # ------------------------------------------------------------------ 3-D augmentation warp (csrc/augment3d.cu)
     def augment3d_workspace(self, n, dhw, device):

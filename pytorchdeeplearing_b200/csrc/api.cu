@@ -198,6 +198,8 @@ int resample_nearest_u8(const uint8_t* src, int D, int H, int W, const double* r
                         int oH, int oW, uint8_t* out, int device, cudaStream_t st);
 int resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc, int n, int oH, int oW, void* out,
                      int out_mode, cudaStream_t st);
+int augment2d(const uint8_t* src, const uint8_t* msrc, const b200seg_aug2d_param* params, int n, long long max_hw,
+              int stages, uint8_t* out, uint8_t* mout, uint8_t* ws, cudaStream_t st);
 long long augment3d_workspace(int n, long long vox);
 int augment3d(const float* x, const void* y, int y_dtype, int n, int D, int H, int W, int C,
               const b200seg_aug3d_param* params, int mode, double cval, int shift, double rescale, int rescale_mode,
@@ -1054,6 +1056,28 @@ int b200seg_resize_linear_u8(const uint8_t* src, const b200seg_resize_src* desc,
                  out_mode);
   B200_DEVICE(device);
   return resize_linear_u8(src, desc, n, oH, oW, out, out_mode, ST(stream));
+}
+
+int64_t b200seg_augment2d_workspace(int64_t out_bytes) { return out_bytes > 0 ? out_bytes : 0; }
+
+int b200seg_augment2d(const uint8_t* src, const uint8_t* msrc, const b200seg_aug2d_param* params, int n,
+                      int64_t max_hw, int stages, uint8_t* out, int64_t out_bytes, uint8_t* mout, void* ws,
+                      int64_t ws_bytes, int device, b200seg_stream stream) {
+  B200_CHECK_ARG(src && params && out, "b200seg_augment2d: null argument");
+  B200_CHECK_ARG(n >= 1 && n <= 65535 && max_hw >= 1 &&
+                     max_hw <= (int64_t)B200SEG_AUG2D_MAX_SIDE * B200SEG_AUG2D_MAX_SIDE && out_bytes >= 1,
+                 "b200seg_augment2d: bad sizes (n %d, max_hw %lld, out_bytes %lld)", n, (long long)max_hw,
+                 (long long)out_bytes);
+  B200_CHECK_ARG(!(stages & ~(B200SEG_AUG2D_HFLIP | B200SEG_AUG2D_VFLIP | B200SEG_AUG2D_BLUR | B200SEG_AUG2D_WARP |
+                              B200SEG_AUG2D_LUT)),
+                 "b200seg_augment2d: bad stages %d", stages);
+  B200_CHECK_ARG((const void*)src != (const void*)out && (!msrc || (const void*)msrc != (const void*)mout) &&
+                     (!mout || (const void*)mout != (const void*)src),
+                 "b200seg_augment2d: outputs alias inputs");
+  B200_CHECK_ARG(!(stages & B200SEG_AUG2D_BLUR) || (ws && ws_bytes >= b200seg_augment2d_workspace(out_bytes)),
+                 "b200seg_augment2d: a blur needs b200seg_augment2d_workspace bytes of workspace");
+  B200_DEVICE(device);
+  return augment2d(src, msrc, params, n, max_hw, stages, out, mout, static_cast<uint8_t*>(ws), ST(stream));
 }
 
 static bool valid_aug3d_sizes(int n, int D, int H, int W) {

@@ -8,7 +8,8 @@ imported later via the same names).  The mask post-processing functions are rebo
 ``GradCAM`` in ``model.visualization`` and ``model.modelResNet`` (so ``Grad_CAM_Visual`` runs on the GPU).
 ``ImageDataGenerator3D`` is rebound in ``dataprocess.Augmentation.
 images_masks_3dtransform`` and ``dataprocess.Augmentation.ImageAugmentation`` (which binds it at import,
-ImageAugmentation.py:1), so an unmodified ``DataAug3D(...).DataAugmentation(...)`` warps on the GPU.  ``uninstall``
+ImageAugmentation.py:1), so an unmodified ``DataAug3D(...).DataAugmentation(...)`` warps on the GPU, and
+``Segmenation_Aug`` in ``dataprocess.AugData`` (the 2-D augmentation).  ``uninstall``
 restores the originals.
 """
 from __future__ import annotations
@@ -35,7 +36,7 @@ _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
             "model.lossescldice", "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet",
             "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation",
-            "dataprocess.utils", "model.visualization")
+            "dataprocess.utils", "model.visualization", "dataprocess.AugData")
 
 
 def install() -> int:
@@ -45,6 +46,7 @@ def install() -> int:
     from .augment import ImageDataGenerator3D
     from . import cldice, postprocess
     from .gradcam import GradCAM
+    from .augment2d import Segmenation_Aug
     table = {n: getattr(nets, n) for n in _NET_NAMES}
     table.update({n: getattr(losses, n) for n in _LOSS_NAMES + _EXT_LOSS_NAMES})
     table.update({n: getattr(metric, n) for n in _METRIC_NAMES})     # per-step accuracy, model/modelVNet.py:582
@@ -53,6 +55,7 @@ def install() -> int:
     table.update({n: getattr(postprocess, n) for n in _POSTPROCESS_NAMES})
     table["ImageDataGenerator3D"] = ImageDataGenerator3D    # dataprocess/Augmentation (DataAug3D)
     table["GradCAM"] = GradCAM                              # model/visualization.py, model/modelResNet.py
+    table["Segmenation_Aug"] = Segmenation_Aug              # dataprocess/AugData.py
     count = 0
     for modname in _MODULES:
         mod = sys.modules.get(modname)

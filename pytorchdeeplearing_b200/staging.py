@@ -18,6 +18,9 @@ resized bit for bit as cv2's INTER_LINEAR (csrc/resize2d.cu) and then staged by 
 
     stager = InputStager(device, (8, 512, 512), max_source_pixels=8 * 1024 * 1024)
     stager.put([cv2.imread(p, 0) for p in paths], [cv2.imread(p, 0) for p in label_paths])   # any sizes
+
+    stager = InputStager(device, (8, 512, 512), max_source_pixels=8 * 1024 * 1024, augment=Segmenation_Aug())
+    stager.put(images, labels)     # + the reference's 2-D augmentation at each source size, before the resize
 """
 from __future__ import annotations
 
@@ -26,7 +29,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import runtime
-from ._abi import RESIZE_SRC_BYTES as _DESC, resize_src_table
+from ._abi import AUG2D_PARAM_BYTES, RESIZE_SRC_BYTES as _DESC, resize_src_table
 
 
 class InputStager:
@@ -37,10 +40,15 @@ class InputStager:
     resizes each to (H, W) as ``cv2.resize(img, (W, H))`` before the z-score; labels are resized the same way before
     the widening.  For square targets this is what the reference's ``datasetModelSegwithopencv`` /
     ``datasetModelClassifywithopencv`` return (image, and label after the trainer's binarisation); those classes pass
-    (H, W) to cv2 as (width, height), so their own assert refuses a non-square target, which the stager accepts."""
+    (H, W) to cv2 as (width, height), so their own assert refuses a non-square target, which the stager accepts.
+
+    ``augment``: a ``Segmenation_Aug`` (augment2d.py), resize mode only.  ``put`` then draws each image's parameters
+    on the host, ships them in the same ragged copy and augments every image (and its label, which must have the
+    image's size) at its source size before the resize: the reference's order, where the augmentation writes its files
+    offline and the dataset resizes and z-scores what it reads back."""
 
     def __init__(self, device, shape: Sequence[int], dtype: torch.dtype = torch.float32, binarize_labels: bool = True,
-                 slots: int = 2, backend=None, max_source_pixels: Optional[int] = None):
+                 slots: int = 2, backend=None, max_source_pixels: Optional[int] = None, augment=None):
         self.device = torch.device(device)
         self.shape = tuple(int(v) for v in shape)
         self.dtype = dtype
@@ -52,6 +60,9 @@ class InputStager:
                 raise ValueError(f"InputStager: the resize mode stages 2-D batches (N, H, W), got shape {self.shape}")
             if self.max_source_pixels < 1:
                 raise ValueError("InputStager: max_source_pixels must be >= 1")
+        self.augment = augment
+        if augment is not None and self.max_source_pixels is None:
+            raise ValueError("InputStager: augment needs the resize mode (max_source_pixels)")
         cuda = self.device.type == "cuda"
         self._stream = torch.cuda.Stream(self.device) if cuda else None
         self._slots = []
@@ -73,6 +84,9 @@ class InputStager:
             ev = torch.cuda.Event() if cuda else None
             self._slots.append(dict(h_img=h_img, h_lab=h_lab, h_src=h_src, d_src=d_src, d_img=d_img, d_lab=d_lab, x=x,
                                     y=y, ready=ev, free=None))
+        if augment is not None:                # the augmented images and labels, and the blur workspace
+            self._d_aug = torch.empty(2 * self.max_source_pixels, dtype=torch.uint8, device=self.device)
+            self._aug_ws = self.be.augment2d_workspace(self._d_aug.numel(), self.device)
         self._put = 0
         self._got = 0
         if self.max_source_pixels is None:
@@ -81,7 +95,7 @@ class InputStager:
             self.h2d_bytes_per_batch = self._pixel_base() + 2 * self.max_source_pixels
 
     def _pixel_base(self) -> int:
-        return 2 * _DESC * self.shape[0]
+        return (2 * _DESC + (AUG2D_PARAM_BYTES if self.augment is not None else 0)) * self.shape[0]
 
     def put(self, images, labels=None) -> None:
         """Queue one batch: uint8 images [N, *spatial] (numpy array or tensor) and, optionally, uint8 labels.  In resize
@@ -154,19 +168,44 @@ class InputStager:
             entries.append((off, t.shape[0], t.shape[1]))
             off += k
         table = resize_src_table(entries)
+        if self.augment is not None:
+            table = table.ljust(2 * _DESC * len(imgs), b"\0") + self._augment_table(s, imgs, labs, entries)
         h[:len(table)].copy_(torch.frombuffer(bytearray(table), dtype=torch.uint8))
         s["used"] = base + off
         s["has_labels"] = labels is not None
         self._launch(s, self._run_ragged)
 
+    def _augment_table(self, s, imgs, labs, entries) -> bytes:
+        """each image's draws -> its ``b200seg_aug2d_param`` bytes; the output goes to the image's own offset of the
+        augmented buffer (its label's likewise)"""
+        from .augment2d import check_pair, draw_params, param_entry
+        n, out, stages = len(imgs), [], 0
+        for i, t in enumerate(imgs):
+            h, w, _ = check_pair(t, labs[i] if labs else None)
+            off = entries[i][0]
+            moff = entries[n + i][0] if labs else -1
+            # the reference writes 3-channel BMPs that the dataset reads back as gray: MotionBlur's fp32 tail as BGR
+            e, f = param_entry(draw_params(), h, w, 1, off, off, moff, max(moff, 0), filter_cn=3)
+            out.append(e)
+            stages |= f
+        s["aug_stages"] = stages
+        s["aug_max_hw"] = max(int(t.numel()) for t in imgs)
+        return b"".join(out)
+
     def _run_ragged(self, s) -> None:
         n, base, d = self.shape[0], self._pixel_base(), s["d_src"]
         d[:s["used"]].copy_(s["h_src"][:s["used"]], non_blocking=True)       # descriptors and pixels in one copy
         pixels = d[base:]
+        if self.augment is not None:
+            params = d[2 * _DESC * n:base]
+            self.be.augment2d(pixels, params, n, s["aug_max_hw"], s["aug_stages"], self._d_aug,
+                              msrc=pixels if s["has_labels"] else None, mout=self._d_aug if s["has_labels"] else None,
+                              ws=self._aug_ws)
+            pixels = self._d_aug
         self.be.resize_linear(pixels, d[:_DESC * n].view(torch.int64).view(n, 2), s["d_img"])
         self.be.stage_images_u8(s["d_img"], s["x"])
         if s["has_labels"]:
-            self.be.resize_linear(pixels, d[_DESC * n:base].view(torch.int64).view(n, 2), s["d_lab"])
+            self.be.resize_linear(pixels, d[_DESC * n:2 * _DESC * n].view(torch.int64).view(n, 2), s["d_lab"])
             self.be.stage_labels_u8(s["d_lab"], s["y"], self.binarize)
 
     def get(self) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
