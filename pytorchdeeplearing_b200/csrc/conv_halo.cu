@@ -17,6 +17,7 @@
 //     epilogue (bias, GroupNorm statistics, residual addend, bf16 NDHWC stores) follow conv_tc.cu.
 // conv_halo_kernel below is the 2-D (1x3x3) form; the 3-D layers take the input-slice-major conv_halo3_kernel.
 // Warp roles (512 threads): warps 0-3 MMA warpgroup, warps 4-7 epilogue, warps 8-15 loaders.
+#include "gn_coef.cuh"
 #include "tc_common.cuh"
 
 namespace b200seg {
@@ -46,17 +47,11 @@ struct HaloArgs {
   int acc_pitch;          // floats per row of the accumulator staging tile in shared memory
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats): the output of this conv is
   // g = dL/d(act) of the layer whose raw output is yfwd; with m = [yfwd*A + B > 0] (A, B = that layer's GroupNorm /
-  // dropout coefficients, derived here from its statistics exactly as gn_cta_coefs does) the epilogue accumulates
+  // dropout coefficients, derived here from its statistics with gn_coefs) the epilogue accumulates
   // sums[n][c][0] += g*m, sums[n][c][1] += g*m*yfwd  (stride 3: [2] = sum yfwd is taken from the forward statistics).
   const bf16* yfwd;       // nullptr: forward statistics mode (stats = [N][Cout][2])
   long long yfld;
-  const double* gstats;   // [N][Cout][2] forward statistics of the layer being differentiated
-  const float* ggamma;
-  const float* gbeta;
-  const float* gscale;    // [N][Cout] dropout scale or nullptr
-  int ggroups;
-  double gm;              // elements per group
-  float geps;
+  GnRef gn;               // the GroupNorm of the layer being differentiated
 };
 
 __device__ __forceinline__ uint64_t make_nosw_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -594,39 +589,6 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
     };
-    // A, B of sample n for the ReLU mask of the backward sums: the same expressions, in the same precision, as
-    // gn_cta_coefs (elementwise.cu), so the mask here equals the one gn_bwd_apply derives later
-    auto load_coefs = [&](int n) {
-      const int cpg = COUT / p.ggroups;
-      if (etid < COUT) {
-        const double* q_ = p.gstats + ((long long)n * COUT + etid) * 2;
-        s_gd[etid] = q_[0];
-        s_gd[COUT + etid] = q_[1];
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (etid < p.ggroups) {
-        double sm = 0.0, sq = 0.0;
-        for (int k_ = 0; k_ < cpg; ++k_) {
-          sm += s_gd[etid * cpg + k_];
-          sq += s_gd[COUT + etid * cpg + k_];
-        }
-        const double mean = sm / p.gm;
-        double var = sq / p.gm - mean * mean;
-        if (var < 0.0) var = 0.0;
-        s_gd[2 * COUT + etid * 2 + 0] = mean;
-        s_gd[2 * COUT + etid * 2 + 1] = rsqrt(var + (double)p.geps);
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (etid < COUT) {
-        const int g_ = etid / cpg;
-        const double mean = s_gd[2 * COUT + g_ * 2 + 0], rstd = s_gd[2 * COUT + g_ * 2 + 1];
-        const double sc = p.gscale ? (double)p.gscale[(long long)n * COUT + etid] : 1.0;
-        const double ga = (double)p.ggamma[etid], be = (double)p.gbeta[etid];
-        s_ab[etid] = (float)(rstd * ga * sc);
-        s_ab[COUT + etid] = (float)((be - mean * rstd * ga) * sc);
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    };
     const bool want_stats = p.stats != nullptr;
     int t_begin, t_end;
     halo3_range(p, t_begin, t_end);
@@ -638,7 +600,11 @@ __global__ void __launch_bounds__(kH3Threads, 1) conv_halo3_kernel(const HaloArg
       if (n != cur_n) {
         if (cur_n >= 0 && want_stats) flush_stats(cur_n);
         cur_n = n;
-        if (bwd) load_coefs(n);
+        // A, B of sample n for the ReLU mask of the backward sums: gn_coefs, so the mask here equals the one
+        // gn_bwd_apply derives later
+        if (bwd)
+          gn_coefs<false, false>(GnNamedBarrier<1, 128>{etid}, p.gn, nullptr, n, COUT, s_gd, nullptr, s_ab,
+                                 s_ab + COUT, nullptr, nullptr, nullptr);
       }
       const int oh = h0 + rh, ow = w0 + rw;
       const bool valid = oh < p.H && ow < p.W;
@@ -828,8 +794,7 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
   p.N = x->n; p.D = x->d; p.H = x->h; p.W = x->w;
   p.Cin = x->c; p.Cout = y->c;
   p.kd = dims == 3 ? 3 : 1;
-  p.yfwd = nullptr; p.yfld = 0; p.gstats = nullptr; p.ggamma = nullptr; p.gbeta = nullptr; p.gscale = nullptr;
-  p.ggroups = 1; p.gm = 1.0; p.geps = 0.f;
+  p.yfwd = nullptr; p.yfld = 0; p.gn = gn_ref(nullptr, 0);
   if (yfwd != nullptr) {
     B200_CHECK_ARG(dims == 3 && gn != nullptr && sums != nullptr && stats == nullptr,
                    "conv_halo: backward statistics need the 3-D input-slice-major kernel");
@@ -838,10 +803,7 @@ int conv_halo(int kind, int dims, const b200seg_tensor* x, const void* wpk, cons
                    "conv_halo: bad forward tensor / GroupNorm reference for the backward statistics");
     p.yfwd = static_cast<const bf16*>(yfwd->ptr);
     p.yfld = yfwd->ld;
-    p.gstats = gn->stats; p.ggamma = gn->gamma; p.gbeta = gn->beta; p.gscale = gn->scale;
-    p.ggroups = gn->groups;
-    p.gm = (double)(y->c / gn->groups) * (double)gn->vox;
-    p.geps = gn->eps;
+    p.gn = gn_ref(gn, y->c);
     p.stats = sums;
   }
   p.tw = (p.W + HT_W - 1) / HT_W;

@@ -44,6 +44,7 @@
 // fill), warp 11 weight streamer.
 #include <type_traits>
 
+#include "gn_coef.cuh"
 #include "tc_common.cuh"
 
 namespace b200seg {
@@ -89,13 +90,7 @@ struct HaloWsArgs {
   // GroupNorm-backward sums fused into the data-gradient epilogue (b200seg_conv_bwdstats; see conv_halo.cu)
   const bf16* yfwd;
   long long yfld;
-  const double* gstats;
-  const float* ggamma;
-  const float* gbeta;
-  const float* gscale;
-  int ggroups;
-  double gm;
-  float geps;
+  GnRef gn;
 };
 
 __device__ __forceinline__ uint64_t ws_nosw_desc(uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -444,38 +439,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
     };
-    // A, B of sample n for the ReLU mask of the backward sums: same expressions and precision as gn_cta_coefs
-    auto load_coefs = [&](int n) {
-      const int C = p.Cout, cpg = C / p.ggroups;
-      for (int c = etid; c < C; c += 128) {
-        const double* q_ = p.gstats + ((long long)n * C + c) * 2;
-        s_gd[c] = q_[0];
-        s_gd[C + c] = q_[1];
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (etid < p.ggroups) {
-        double sm = 0.0, sq = 0.0;
-        for (int k_ = 0; k_ < cpg; ++k_) {
-          sm += s_gd[etid * cpg + k_];
-          sq += s_gd[C + etid * cpg + k_];
-        }
-        const double mean = sm / p.gm;
-        double var = sq / p.gm - mean * mean;
-        if (var < 0.0) var = 0.0;
-        s_gd[2 * C + etid * 2 + 0] = mean;
-        s_gd[2 * C + etid * 2 + 1] = rsqrt(var + (double)p.geps);
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      for (int c = etid; c < C; c += 128) {
-        const int g_ = c / cpg;
-        const double mean = s_gd[2 * C + g_ * 2 + 0], rstd = s_gd[2 * C + g_ * 2 + 1];
-        const double sc = p.gscale ? (double)p.gscale[(long long)n * C + c] : 1.0;
-        const double ga = (double)p.ggamma[c], be = (double)p.gbeta[c];
-        s_ab[c] = (float)(rstd * ga * sc);
-        s_ab[C + c] = (float)((be - mean * rstd * ga) * sc);
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    };
     for (int u = u_begin; u < u_end;) {
       const WsSeg sg = ws_segment(p, u, u_end);
       const int n = sg.n, d0 = sg.d0, nd = sg.nd;
@@ -484,7 +447,10 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_halows_kernel(const HaloWs
       if (n != cur_n) {
         if (cur_n >= 0 && want_stats) flush_stats(cur_n);
         cur_n = n;
-        if constexpr (BWD) load_coefs(n);
+        // A, B of sample n for the ReLU mask of the backward sums (gn_coefs, as gn_bwd_apply derives them)
+        if constexpr (BWD)
+          gn_coefs<false, false>(GnNamedBarrier<1, 128>{etid}, p.gn, nullptr, n, p.Cout, s_gd, nullptr, s_ab,
+                                 s_ab + p.Cout, nullptr, nullptr, nullptr);
       }
       int oh = sg.h0 + rh, ow = sg.w0 + rw;
       if constexpr (FLAT) {
@@ -743,8 +709,7 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
     p.tw = (p.W + WS_TW - 1) / WS_TW;
     p.th = (p.H + WS_TH - 1) / WS_TH;
   }
-  p.yfwd = nullptr; p.yfld = 0; p.gstats = nullptr; p.ggamma = nullptr; p.gbeta = nullptr; p.gscale = nullptr;
-  p.ggroups = 1; p.gm = 1.0; p.geps = 0.f;
+  p.yfwd = nullptr; p.yfld = 0; p.gn = gn_ref(nullptr, 0);
   if (yfwd != nullptr) {
     B200_CHECK_ARG(gn != nullptr && sums != nullptr && stats == nullptr && same_geom(yfwd, y) &&
                        yfwd->dtype == B200SEG_BF16 && (yfwd->ld % 8) == 0 && al16w(yfwd->ptr) && gn->groups > 0 &&
@@ -752,10 +717,7 @@ int conv_halows(int kind, int dims, const b200seg_tensor* x, const void* wpk, co
                    "conv_halows: bad forward tensor / GroupNorm reference for the backward statistics");
     p.yfwd = static_cast<const bf16*>(yfwd->ptr);
     p.yfld = yfwd->ld;
-    p.gstats = gn->stats; p.ggamma = gn->gamma; p.gbeta = gn->beta; p.gscale = gn->scale;
-    p.ggroups = gn->groups;
-    p.gm = (double)(y->c / gn->groups) * (double)gn->vox;
-    p.geps = gn->eps;
+    p.gn = gn_ref(gn, y->c);
     p.stats = sums;
   }
   // NT = 64 columns per MMA (narrower groups re-read A for less work).  Two output slices share each streamed tap

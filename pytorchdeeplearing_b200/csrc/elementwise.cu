@@ -269,88 +269,16 @@ __global__ void gn_finalize_kernel(const double* __restrict__ stats, const float
       s += p[0];
       q += p[1];
     }
-    double mean = s / m;
-    double var = q / m - mean * mean;
-    if (var < 0.0) var = 0.0;
-    double rstd = rsqrt(var + (double)eps);
+    double mean, rstd;
+    gn_mean_rstd(s, q, m, eps, mean, rstd);
     double sc = scale ? (double)scale[(long long)n * C + c] : 1.0;
     double ga = gamma[c], be = beta[c];
-    coef[((long long)n * C + c) * 2 + 0] = (float)(rstd * ga * sc);
-    coef[((long long)n * C + c) * 2 + 1] = (float)((be - mean * rstd * ga) * sc);
+    coef[((long long)n * C + c) * 2 + 0] = (float)gn_a(rstd, ga, sc);
+    coef[((long long)n * C + c) * 2 + 1] = (float)gn_b(mean, rstd, ga, be, sc);
     if (c == g * cpg) {
       mr[((long long)n * groups + g) * 2 + 0] = (float)mean;
       mr[((long long)n * groups + g) * 2 + 1] = (float)rstd;
     }
-  }
-}
-
-
-template <int VEC>
-__device__ __forceinline__ void gn_coef_from_stats(const GnRef& r, int n, int C, int c0, float* A, float* B,
-                                                   double* MU, double* RS) {
-  const int cpg = C / r.groups;
-  int last_g = -1;
-  double mean = 0.0, rstd = 0.0;
-#pragma unroll
-  for (int j = 0; j < VEC; ++j) {
-    const int c = c0 + j;
-    const int g = c / cpg;
-    if (g != last_g) {
-      double s = 0.0, q = 0.0;
-      for (int k = 0; k < cpg; ++k) {
-        const double* p = r.stats + ((long long)n * C + g * cpg + k) * 2;
-        s += p[0];
-        q += p[1];
-      }
-      mean = s / r.m;
-      double var = q / r.m - mean * mean;
-      if (var < 0.0) var = 0.0;
-      rstd = rsqrt(var + (double)r.eps);
-      last_g = g;
-    }
-    const double sc = r.scale ? (double)r.scale[(long long)n * C + c] : 1.0;
-    const double ga = r.gamma[c], be = r.beta[c];
-    A[j] = (float)(rstd * ga * sc);
-    B[j] = (float)((be - mean * rstd * ga) * sc);
-    if (MU) MU[j] = mean;
-    if (RS) RS[j] = rstd;
-  }
-}
-
-// P, Q, R of  dy = g*m*P + y*Q + R  for the thread's channels, from the backward sums (SURVEY.md App. G)
-template <int VEC>
-__device__ __forceinline__ void gn_bwd_coef_from_sums(const GnRef& r, const double* __restrict__ sums, int n, int C,
-                                                      int c0, const double* MU, const double* RS, float* P, float* Q,
-                                                      float* R, double* QD = nullptr, double* RD = nullptr) {
-  const int cpg = C / r.groups;
-  int last_g = -1;
-  double m1 = 0.0, m2 = 0.0;
-#pragma unroll
-  for (int j = 0; j < VEC; ++j) {
-    const int c = c0 + j;
-    const int g = c / cpg;
-    const double mu = MU[j], rs = RS[j];
-    if (g != last_g) {
-      double sa = 0.0, sax = 0.0;
-      for (int k = 0; k < cpg; ++k) {
-        const int ck = g * cpg + k;
-        const double sk = r.scale ? (double)r.scale[(long long)n * C + ck] : 1.0;
-        const double* p = sums + ((long long)n * C + ck) * 3;
-        const double s1 = p[0] * sk, s2 = p[1] * sk;
-        const double gk = r.gamma[ck];
-        sa += gk * s1;
-        sax += gk * rs * (s2 - mu * s1);
-      }
-      m1 = sa / r.m;
-      m2 = sax / r.m;
-      last_g = g;
-    }
-    const double sc = r.scale ? (double)r.scale[(long long)n * C + c] : 1.0;
-    P[j] = (float)(rs * (double)r.gamma[c] * sc);
-    Q[j] = (float)(-rs * rs * m2);
-    R[j] = (float)(-rs * m1 + rs * rs * mu * m2);
-    if (QD) QD[j] = -rs * rs * m2;
-    if (RD) RD[j] = -rs * m1 + rs * rs * mu * m2;
   }
 }
 
@@ -407,8 +335,10 @@ __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1,
     double* s_d = s_dyn;                                                  // scratch doubles
     float* s_f = reinterpret_cast<float*>(s_d + gn_cta_doubles(C, gn1.groups > gn2.groups ? gn1.groups : gn2.groups, false));
     float* s_cf = s_f + 3 * C;                                            // [4][C]: A1, B1, A2, B2
-    gn_cta_coefs<false>(gn1, nullptr, n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
-    if (y2 != nullptr) gn_cta_coefs<false>(gn2, nullptr, n, C, s_d, s_f, s_cf + 2 * C, s_cf + 3 * C, nullptr, nullptr, nullptr);
+    gn_coefs<false, true>(GnCta(), gn1, nullptr, n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
+    if (y2 != nullptr)
+      gn_coefs<false, true>(GnCta(), gn2, nullptr, n, C, s_d, s_f, s_cf + 2 * C, s_cf + 3 * C, nullptr, nullptr,
+                            nullptr);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
       A1[j] = s_cf[c0 + j];
@@ -510,7 +440,7 @@ __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const 
   float A[VEC], B[VEC];
   float f1[VEC], f2[VEC], f3[VEC];
   if (gn.stats != nullptr) {
-    gn_cta_coefs<false>(gn, nullptr, n, C, s_cd, s_cfl, s_ab, s_ab + C, nullptr, nullptr, nullptr);
+    gn_coefs<false, true>(GnCta(), gn, nullptr, n, C, s_cd, s_cfl, s_ab, s_ab + C, nullptr, nullptr, nullptr);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
       A[j] = s_ab[c0 + j];
@@ -648,23 +578,23 @@ __global__ void gn_bwd_finalize_kernel(const double* __restrict__ sums, const fl
         const double* p = sums + ((long long)n * C + cj) * 3;
         const double s1 = p[0] * sj, s2 = p[1] * sj;
         const double gj = gamma[cj];
-        sa += gj * s1;
-        sax += gj * r * (s2 - mu * s1);
+        sa += gn_m1_term(gj, s1);
+        sax += gn_m2_term(mu, r, gj, s1, s2);
       }
       const double m1 = sa / m, m2 = sax / m;
       const double sc = scale ? (double)scale[(long long)n * C + c] : 1.0;
       const double* p = sums + ((long long)n * C + c) * 3;
       const double s1 = p[0] * sc, s2 = p[1] * sc, s3 = p[2];
-      const double P = r * ga * sc;
-      const double Q = -r * r * m2;
-      const double R = -r * m1 + r * r * mu * m2;
+      const double P = gn_a(r, ga, sc);
+      const double Q = gn_q(r, m2);
+      const double R = gn_r(mu, r, m1, m2);
       float* o = coef3 + ((long long)n * C + c) * 3;
       o[0] = (float)P;
       o[1] = (float)Q;
       o[2] = (float)R;
       db += s1;
-      dg += r * (s2 - mu * s1);
-      dbi += r * ga * s1 + Q * s3 + R * vox;
+      dg += gn_dgamma(mu, r, s1, s2);
+      dbi += gn_dbias(r, ga, s1, s3, Q, R, vox);
     }
     dgamma[c] += (float)dg;
     dbeta[c] += (float)db;
@@ -690,8 +620,8 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
     double* s_d = s_dyn;
     float* s_f = reinterpret_cast<float*>(s_d + gn_cta_doubles(C, gn.groups, true));
     float* s_c5 = s_f + 3 * C;                            // [5][C]: A, B, P, Q, R
-    const double* grp = gn_cta_coefs<true>(gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C, s_c5 + 3 * C,
-                                           s_c5 + 4 * C);
+    const double* grp = gn_coefs<true, true>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
+                                             s_c5 + 3 * C, s_c5 + 4 * C);
     // parameter gradients (d gamma, d beta, d bias): ONE block per sample adds its sample's share from the
     // coefficients it has just derived (no serial loop over the batch at the tail of the grid); fp32 atomics over N
     if (blockIdx.x == gridDim.x - 1) param_grads_of_sample(gn, sums, grp, s_f, n, C, dgamma, dbeta, dbias);
@@ -770,7 +700,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
   const T* gb = g + (long long)n * V * ldg + c0;
   float A[VEC], B[VEC];
   // ---------------------------------------------------------------- phase 1: per-(n, c) sums
-  gn_cta_coefs<false>(gn, nullptr, n, C, s_d, s_f, s_c5, s_c5 + C, nullptr, nullptr, nullptr);
+  gn_coefs<false, true>(GnCta(), gn, nullptr, n, C, s_d, s_f, s_c5, s_c5 + C, nullptr, nullptr, nullptr);
   float f1[VEC], f2[VEC], f3[VEC];
 #pragma unroll
   for (int j = 0; j < VEC; ++j) {
@@ -831,8 +761,8 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
   __syncthreads();
   // ---------------------------------------------------------------- phase 2: dy and the parameter gradients
   float P[VEC], Q[VEC], R[VEC];
-  const double* grp = gn_cta_coefs<true>(gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C, s_c5 + 3 * C,
-                                         s_c5 + 4 * C);
+  const double* grp = gn_coefs<true, true>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
+                                           s_c5 + 3 * C, s_c5 + 4 * C);
   if (blockIdx.x == gridDim.x - 1) param_grads_of_sample(gn, sums, grp, s_f, n, C, dgamma, dbeta, dbias);
 #pragma unroll
   for (int j = 0; j < VEC; ++j) {
@@ -1074,20 +1004,6 @@ int ew_gn_finalize(const double* stats, const float* gamma, const float* beta, c
   return B200SEG_OK;
 }
 
-static GnRef make_gnref(const b200seg_gn* g, int C) {
-  GnRef r;
-  if (g == nullptr || g->stats == nullptr) {
-    r.stats = nullptr; r.gamma = nullptr; r.beta = nullptr; r.scale = nullptr; r.groups = 1; r.m = 1.0; r.eps = 0.f;
-    r.sum_y_from_stats = 0;
-    return r;
-  }
-  r.stats = g->stats; r.gamma = g->gamma; r.beta = g->beta; r.scale = g->scale; r.groups = g->groups;
-  r.m = (double)(C / g->groups) * (double)g->vox;
-  r.eps = g->eps;
-  r.sum_y_from_stats = 0;
-  return r;
-}
-
 int ew_apply(const b200seg_tensor* y1, const float* c1, const b200seg_gn* g1, const b200seg_tensor* y2,
              const float* c2, const b200seg_gn* g2, const b200seg_tensor* res, const b200seg_tensor* out, int device,
              cudaStream_t s) {
@@ -1106,7 +1022,7 @@ int ew_apply(const b200seg_tensor* y1, const float* c1, const b200seg_gn* g1, co
     const size_t smem = (g1 && g1->stats) ? gn_cta_doubles(C, mg, false) * sizeof(double) + (size_t)7 * C * sizeof(float) : 0;
     launch_k(apply_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(y1->ptr), y1->ld, c1, y2 ? static_cast<const T*>(y2->ptr) : nullptr, y2 ? y2->ld : 0, c2,
         res ? static_cast<const T*>(res->ptr) : nullptr, res ? res->ld : 0, static_cast<T*>(out->ptr), out->ld, C, V,
-        make_gnref(g1, C), make_gnref(g2, C));
+        gn_ref(g1, C), gn_ref(g2, C));
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
@@ -1132,10 +1048,10 @@ int ew_gn_bwd_reduce(const b200seg_tensor* g, const b200seg_tensor* y, const flo
     const size_t base = (gn && gn->stats) ? full : (size_t)3 * C * sizeof(double);
     if (deep)
       launch_k(gn_bwd_reduce_kernel<T, VEC, true>, grid, 256, staged ? staged_bytes : base, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, coef, sums, C, V,
-          make_gnref(gn, C), staged);
+          gn_ref(gn, C), staged);
     else
       launch_k(gn_bwd_reduce_kernel<T, VEC, false>, grid, 256, staged ? staged_bytes : base, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, coef, sums, C, V,
-          make_gnref(gn, C), staged);
+          gn_ref(gn, C), staged);
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
@@ -1166,7 +1082,7 @@ int ew_gn_bwd_apply(const b200seg_tensor* g, const b200seg_tensor* y, const floa
     dim3 grid(ew_blocks(V, G, y->n, device, 3), y->n);
     const int groups = (gn && gn->stats) ? gn->groups : 1;
     const size_t smem = (gn && gn->stats) ? gn_cta_doubles(C, groups, true) * sizeof(double) + (size_t)8 * C * sizeof(float) : 0;
-    GnRef gref = make_gnref(gn, C);
+    GnRef gref = gn_ref(gn, C);
     gref.sum_y_from_stats = sum_y_from_stats;
     launch_k(gn_bwd_apply_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld,
                                                      static_cast<const T*>(y->ptr), y->ld, coef, coef3,
@@ -1214,7 +1130,7 @@ int ew_gn_bwd_fused(const b200seg_tensor* g, const b200seg_tensor* y, const b200
     B200_CHECK_ARG(bx >= 1 && (long long)bx * y->n <= sms, "gn_bwd_fused: batch too large for a resident grid");
     dim3 grid(bx, y->n);
     launch_k(gn_bwd_fused_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, static_cast<T*>(dy->ptr), dy->ld,
-        sums, counter, C, V, make_gnref(gn, C), y->n, dgamma, dbeta, dbias);
+        sums, counter, C, V, gn_ref(gn, C), y->n, dgamma, dbeta, dbias);
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;

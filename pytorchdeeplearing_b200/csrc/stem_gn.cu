@@ -9,7 +9,7 @@
 //   STATS   per-(n, c) sum y, sum y^2 of both branches (fp64; the stem epilogue's order and convention: sums of the
 //           fp32 accumulators, lanes -> warps -> one fp64 atomic per CTA and sample)
 //   APPLY   out = relu(y_a*A_a + B_a) + relu(y_b*A_b + B_b), A/B derived per CTA from the statistics, gamma, beta
-//           and the dropout scale exactly as apply_kernel does (gn_cta_coefs), written into a pitched buffer
+//           and the dropout scale exactly as apply_kernel does (gn_coefs), written into a pitched buffer
 //   BSUMS   per-(n, c) sum g*m, sum g*m*y, sum y of both branches (m = ReLU mask), the layout gn_bwd_apply_gn reads
 //   BWD     dy = g*m*P + y*Q + R per branch (rounded to bf16 as the stored dy is), kept on chip and fed straight into
 //           both stem weight gradients (the fragment path of wgrad_stem_mma_kernel); d gamma, d beta and both bias
@@ -166,9 +166,10 @@ __global__ void __launch_bounds__(SM_THREADS, MODE == SG_BWD ? 1 : 2)
   // coefficients of sample n, both branches, into s_cf (every thread calls: block barriers).  The lanes read them
   // from shared memory where they are used: the registers go to the prefetched image window and the accumulators.
   auto load_coefs = [&](int n) {
-    gn_cta_coefs<BWD>(p.gna, p.sums_a, n, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C, s_cf + 4 * C);
+    gn_coefs<BWD, true>(GnCta(), p.gna, p.sums_a, n, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C,
+                        s_cf + 4 * C);
     float* cb = s_cf + 5 * C;
-    gn_cta_coefs<BWD>(p.gnb, p.sums_b, n, C, s_d, s_f, cb, cb + C, cb + 2 * C, cb + 3 * C, cb + 4 * C);
+    gn_coefs<BWD, true>(GnCta(), p.gnb, p.sums_b, n, C, s_d, s_f, cb, cb + C, cb + 2 * C, cb + 3 * C, cb + 4 * C);
   };
   // coefficient k (0..4 = A, B, P, Q, R) of branch b for the lane's channel pair of n-tile nt
   auto cf = [&](int b, int k, int nt) {
@@ -457,12 +458,12 @@ __global__ void __launch_bounds__(SM_THREADS, MODE == SG_BWD ? 1 : 2)
     // d gamma, d beta, d bias of both branches: one CTA per sample, from the sums (as gn_bwd_apply_kernel)
     for (int s = blockIdx.x; s < g.N; s += gridDim.x) {
       __syncthreads();
-      const double* grp = gn_cta_coefs<true>(p.gna, p.sums_a, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C,
-                                             s_cf + 3 * C, s_cf + 4 * C);
+      const double* grp = gn_coefs<true, true>(GnCta(), p.gna, p.sums_a, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C,
+                                               s_cf + 3 * C, s_cf + 4 * C);
       param_grads_of_sample(p.gna, p.sums_a, grp, s_f, s, C, p.dgamma, p.dbeta, p.dba);
       __syncthreads();
-      grp = gn_cta_coefs<true>(p.gnb, p.sums_b, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C,
-                               s_cf + 4 * C);
+      grp = gn_coefs<true, true>(GnCta(), p.gnb, p.sums_b, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C,
+                                 s_cf + 4 * C);
       param_grads_of_sample(p.gnb, p.sums_b, grp, s_f, s, C, p.dgamma, p.dbeta, p.dbb);
     }
   }
@@ -479,15 +480,6 @@ int stem_gn_supported(const b200seg_tensor* x, int cout, int dims) {
   y.dtype = B200SEG_BF16;
   StemGeom g;
   return stem_mma_geom(x, &y, &g) ? 1 : 0;
-}
-
-static GnRef sg_gnref(const b200seg_gn* gn) {
-  GnRef r;
-  r.stats = gn->stats; r.gamma = gn->gamma; r.beta = gn->beta; r.scale = gn->scale; r.groups = gn->groups;
-  r.m = (double)(SG_C / gn->groups) * (double)gn->vox;
-  r.eps = gn->eps;
-  r.sum_y_from_stats = 0;
-  return r;
 }
 
 template <int MODE>
@@ -540,8 +532,8 @@ int stem_gn(int mode, const b200seg_tensor* x, const void* wa, const float* ba, 
     return stem_gn_launch<SG_STATS>(x, p, device, st);
   }
   B200_CHECK_ARG(sg_gn_ok(gna, x) && sg_gn_ok(gnb, x), "b200seg_stem_gn: bad GroupNorm reference (8 groups, vox = D*H*W)");
-  p.gna = sg_gnref(gna);
-  p.gnb = sg_gnref(gnb);
+  p.gna = gn_ref(gna, SG_C);
+  p.gnb = gn_ref(gnb, SG_C);
   if (mode == SG_APPLY) {
     B200_CHECK_ARG(sg_act_ok(out, x) && (out->ld % 2) == 0, "b200seg_stem_gn_apply: bad output tensor");
     p.out = static_cast<bf16*>(out->ptr);

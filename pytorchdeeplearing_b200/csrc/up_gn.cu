@@ -7,7 +7,7 @@
 //
 //   STATS   per-(n, c) sum y, sum y^2: the PW_MMA epilogue's order and partials (same tile walk, lanes -> warps -> one
 //           fp64 atomic per CTA and sample)
-//   APPLY   out = relu(y*A + B), A/B from the statistics, gamma, beta and dropout scale (gn_cta_coefs), written into a
+//   APPLY   out = relu(y*A + B), A/B from the statistics, gamma, beta and dropout scale (gn_coefs), written into a
 //           pitched buffer
 //   BSUMS   per-(n, c) sum g*m, sum g*m*y, sum y (m = ReLU mask), the layout gn_bwd_apply_gn reads
 //   BWD     dy = g*m*P + y*Q + R, rounded to bf16 as the stored dy is, kept on chip: it feeds the data gradient to the
@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(PW_THREADS, 1) up_gn_kernel(const __grid_const
     __syncthreads();
   };
   auto coefs = [&](long long n) {
-    gn_cta_coefs<false>(p.gn, nullptr, (int)n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
+    gn_coefs<false, true>(GnCta(), p.gn, nullptr, (int)n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
   };
 
   const long long tiles = p.NV / PW_TILE;
@@ -361,7 +361,8 @@ __global__ void __launch_bounds__(PW_THREADS, 1) up_gn_bwd_kernel(const __grid_c
 #pragma unroll
   for (int ct = 0; ct < CT; ++ct) accw[ct][0] = accw[ct][1] = accw[ct][2] = accw[ct][3] = 0.f;
   auto coefs = [&](long long n) {
-    gn_cta_coefs<true>(p.gn, p.sums, (int)n, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C, s_cf + 4 * C);
+    gn_coefs<true, true>(GnCta(), p.gn, p.sums, (int)n, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C,
+                         s_cf + 4 * C);
   };
   auto cf = [&](int k, int nt) { return *reinterpret_cast<const float2*>(s_cf + k * C + nt * 8 + 2 * tq); };
 
@@ -498,8 +499,8 @@ __global__ void __launch_bounds__(PW_THREADS, 1) up_gn_bwd_kernel(const __grid_c
   // d gamma, d beta, d bias: one CTA per sample, from the sums (as gn_bwd_apply_kernel)
   for (int s = blockIdx.x; s < p.N; s += gridDim.x) {
     __syncthreads();
-    const double* grp = gn_cta_coefs<true>(p.gn, p.sums, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C, s_cf + 3 * C,
-                                           s_cf + 4 * C);
+    const double* grp = gn_coefs<true, true>(GnCta(), p.gn, p.sums, s, C, s_d, s_f, s_cf, s_cf + C, s_cf + 2 * C,
+                                             s_cf + 3 * C, s_cf + 4 * C);
     param_grads_of_sample(p.gn, p.sums, grp, s_f, s, C, p.dgamma, p.dbeta, p.dbias);
   }
 }
@@ -574,11 +575,7 @@ int up_gn(int mode, const b200seg_tensor* x, const void* w, const float* bias, c
     return ug_launch(up_gn_kernel<UG_STATS>, p, ug_smem(UG_STATS), tiles, device, st, attr);
   }
   B200_CHECK_ARG(ug_gn_ok(gn, x), "b200seg_up_gn: bad GroupNorm reference (8 groups, vox = the fine grid's D*H*W)");
-  p.gn.stats = gn->stats; p.gn.gamma = gn->gamma; p.gn.beta = gn->beta; p.gn.scale = gn->scale;
-  p.gn.groups = gn->groups;
-  p.gn.m = (double)(UG_C / gn->groups) * (double)gn->vox;
-  p.gn.eps = gn->eps;
-  p.gn.sum_y_from_stats = 0;
+  p.gn = gn_ref(gn, UG_C);
   if (mode == 1) {
     B200_CHECK_ARG(ug_fine_ok(out, x), "b200seg_up_gn_apply: bad output tensor (bf16, 16 channels, the fine grid, 16-byte aligned rows)");
     p.out = static_cast<bf16*>(out->ptr);
