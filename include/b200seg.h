@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define B200SEG_VERSION 200
+#define B200SEG_VERSION 201
 
 #define B200SEG_OK 0
 #define B200SEG_EINVAL (-1)   /* bad argument / unsupported combination */
@@ -197,14 +197,22 @@ int b200seg_apply(const b200seg_tensor* y1, const float* coef1, const b200seg_te
 /* Fused-coefficient forms: the kernels derive A, B (and the backward P, Q, R, d gamma, d beta, d bias) for their
  * own channels from the fp64 statistics, so no finalize launches are needed.  `b200seg_gn` names one GroupNorm
  * application: statistics [N][C][2] written by b200seg_conv, affine parameters, optional dropout scale [N][C]. */
+/* activation after the norm and dropout (b200seg_gn.act) */
+#define B200SEG_ACT_RELU 0   /* nn.ReLU */
+#define B200SEG_ACT_LEAKY 1  /* nn.LeakyReLU(0.01): v > 0 ? v : v * 0.01f; backward g > 0 ? g : g * 0.01f by the sign of
+                                the pre-activation (leaky_relu_backward).  Only the elementwise GroupNorm entry points
+                                (b200seg_apply_gn, b200seg_gn_bwd_reduce_gn, b200seg_gn_bwd_apply_gn,
+                                b200seg_gn_bwd_fused_gn) take it; the fused families (b200seg_conv_bwdstats,
+                                b200seg_stem_gn_*, b200seg_up_gn_*) return B200SEG_EINVAL for act != RELU. */
 typedef struct b200seg_gn {
   const double* stats;
   const float* gamma;
   const float* beta;
   const float* scale;
-  int32_t groups;
+  int32_t groups;  /* 8 for nn.GroupNorm(8, C); C for nn.InstanceNorm3d(C, affine=True) (C <= 512) */
   int64_t vox;     /* voxels per sample of the normalised tensor */
   float eps;
+  int32_t act;     /* B200SEG_ACT_*: fills the padding after eps, sizeof is unchanged */
 } b200seg_gn;
 int b200seg_apply_gn(const b200seg_tensor* y1, const b200seg_gn* gn1, const b200seg_tensor* y2, const b200seg_gn* gn2,
                      const b200seg_tensor* res, const b200seg_tensor* out, int device, b200seg_stream stream);
@@ -743,6 +751,28 @@ int b200seg_gradcam_layer(const b200seg_tensor* act, const b200seg_tensor* grad,
                           void* workspace, int64_t workspace_bytes, float* out, int device, b200seg_stream stream);
 int b200seg_gradcam_scale(float* out, int n, int H, int W, void* workspace, int64_t workspace_bytes, int device,
                           b200seg_stream stream);
+
+/* ---- voxelmorph's SpatialTransformer as VNet3dRegistration uses it (networks/VNet3dregistration.py:6-45,171-206):
+ * F.grid_sample(src, new_locs, align_corners=True, padding_mode='zeros') at new_locs built from the displacement
+ * field.  ddf: fp32 channels-last [N][D][H][W][3] (channel i displaces axis i: 0 = D, 1 = H, 2 = W), as the head
+ * writes it.  Per voxel (d, h, w) and axis i with grid g = (d, h, w) and s_i = (D, H, W)[i] > 1, in fp32 in this order
+ * and without FMA contraction:
+ *   loc = g_i + ddf_i,   nrm = 2 * (loc / (s_i - 1) - 0.5),   u_i = ((nrm + 1) / 2) * (s_i - 1)
+ * (the reference's normalisation, then grid_sample's align-corners unnormalisation; the channel reversal
+ * [..., [2, 1, 0]] makes u_2 the x coordinate over W and u_0 the z coordinate over D).
+ * b200seg_warp3d writes, for every channel, moved_image = trilinear sample of image at u (torch's floor cell and
+ * weights, the eight corners in grid_sample's order, out-of-volume corners read 0) and moved_label = label at
+ * nearbyint(u) (round half to even; 0 outside the volume).  image / moved_image: fp32 NCDHW-contiguous [N][Ci][D][H][W],
+ * label / moved_label: fp32 [N][Cl][D][H][W]; either pair may be NULL (Ci or Cl = 0).
+ * b200seg_warp3d_bwd: gddf [N][D][H][W][3] = d loss / d ddf from gmoved (d loss / d moved_image, NCDHW) through the
+ * trilinear path (grid_sample's grid gradient: the one-sided derivative of the floor cell, summed over the channels in
+ * order, times (s_i - 1) / 2, then the normalisation's 2 / (s_i - 1)), plus addend (same layout, or NULL).  The label
+ * path passes no gradient, and there is none to image or label.  One thread per voxel: no atomics, reruns are
+ * bit-identical.  D, H, W >= 2; N * D * H * W < 2^31. */
+int b200seg_warp3d(const float* ddf, const float* image, int ci, const float* label, int cl, int N, int D, int H, int W,
+                   float* moved_image, float* moved_label, int device, b200seg_stream stream);
+int b200seg_warp3d_bwd(const float* ddf, const float* image, int ci, const float* gmoved, const float* addend, int N,
+                       int D, int H, int W, float* gddf, int device, b200seg_stream stream);
 int b200seg_gradcam_target(const float* logits, int n, int k, int target, float* dlogits, int64_t* category,
                            int device, b200seg_stream stream);
 

@@ -16,7 +16,9 @@ module raises as shipped, so its evident intent runs here, with four documented 
 ``MorphologicalOperation``, ``GetLargestConnectedCompontBoundingbox``), and Grad-CAM of ResNet2d
 (``grad_cam`` and the reference-named ``GradCAM`` of ``model/visualization.py``), and the 2-D data augmentation of
 ``dataprocess/AugData.py`` (``Segmenation_Aug``: cv2's flips, blurs, warp and table byte for byte, offline through
-``DataAugmentation`` or per training step through ``transform_batch`` and ``InputStager(augment=...)``).
+``DataAugmentation`` or per training step through ``transform_batch`` and ``InputStager(augment=...)``), and
+voxelmorph's SpatialTransformer as ``networks/VNet3dregistration.py`` uses it (``warp3d``: the trilinear image and
+nearest label warp by a displacement field, with d loss / d ddf).
 
     from pytorchdeeplearing_b200 import VNet3d, MutilDiceLoss      # same ctor signatures
     import pytorchdeeplearing_b200 as b200; b200.install()         # or patch the reference in place
@@ -25,7 +27,8 @@ Host code is Python/PyTorch (device memory, streams, torch.distributed); every F
 hand-written CUDA kernels behind the C ABI of ``include/b200seg.h``.
 """
 from .runtime import (set_precision, get_precision, enable_data_parallel, disable_data_parallel)
-from .networks import VNet3d, VNet2d, UNet3d, UNet3dthin, UNet2d, ResNet3d, ResNet2d, initialize_weights
+from .networks import (VNet3d, VNet2d, UNet3d, UNet3dthin, UNet2d, ResNet3d, ResNet2d, VNet3dRegistration,
+                       initialize_weights)
 from .losses import (BinaryDiceLoss, BinaryCrossEntropyLoss, BinaryFocalLoss, BinaryCrossEntropyDiceLoss,
                      BinaryDiceFocalLoss, MutilCrossEntropyLoss, MutilFocalLoss, MutilDiceLoss,
                      MutilCrossEntropyDiceLoss, BinaryJaccardLoss, BinaryELDiceLoss, BinarySSLoss, BinaryTverskyLoss,
@@ -44,8 +47,9 @@ from .postprocess import (largest_component, binary_morphology, label_bbox, GetL
                           MorphologicalOperation, GetLargestConnectedCompontBoundingbox)
 from .gradcam import grad_cam, GradCAM
 from .augment2d import Segmenation_Aug
+from .warp import warp3d
 
-__all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
+__all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "ResNet2d", "VNet3dRegistration", "initialize_weights", "FusedAdamW", "FusedAdam", "dice_coeff",
            "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "seg_metrics3d", "Seg_Metirc3d", "predict",
            "predict_mask",
            "sliding_window_mask", "inference3d", "inference_patch3d", "resample3d", "spacing_size", "resize2d", "inference2d", "ImageDataGenerator3D", "InputStager", "stage_batch", "set_precision", "get_precision",
@@ -56,4 +60,5 @@ __all__ = ["VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet3d", "Re
            "MutilELDiceLoss", "LovaszLoss", "BinaryLovaszLoss", "lovasz_hinge", "SSIM", "SSIM3D", "ssim", "ssim3D",
            "soft_skeletonize", "norm_intersection", "Binary_Soft_cldice_loss", "Mutil_Soft_cldice_loss",
            "largest_component", "binary_morphology", "label_bbox", "GetLargestConnectedCompont",
-           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox", "grad_cam", "GradCAM", "Segmenation_Aug"]
+           "MorphologicalOperation", "GetLargestConnectedCompontBoundingbox", "grad_cam", "GradCAM", "Segmenation_Aug",
+           "warp3d"]

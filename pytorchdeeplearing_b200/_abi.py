@@ -48,9 +48,13 @@ class PackDesc(C.Structure):   # include/b200seg.h: struct b200seg_pack_desc
                 ("N1", C.c_int32), ("flip", C.c_int32), ("block_start", C.c_int32), ("nblocks", C.c_int32)]
 
 
+# activation after the norm (B200SEG_ACT_*): nn.ReLU, nn.LeakyReLU(0.01)
+ACT_RELU, ACT_LEAKY = 0, 1
+
+
 class GnDesc(C.Structure):     # include/b200seg.h: struct b200seg_gn
     _fields_ = [("stats", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("scale", C.c_void_p),
-                ("groups", C.c_int32), ("vox", C.c_int64), ("eps", C.c_float)]
+                ("groups", C.c_int32), ("vox", C.c_int64), ("eps", C.c_float), ("act", C.c_int32)]
 
 
 _PT = C.POINTER(TensorDesc)
@@ -167,6 +171,8 @@ _SIGNATURES = {
     "b200seg_gradcam_layer": ([_PT, _PT, _i, _i, _i, _i, _vp, _i64, _vp, _i, _vp], C.c_int),
     "b200seg_gradcam_scale": ([_vp, _i, _i, _i, _vp, _i64, _i, _vp], C.c_int),
     "b200seg_gradcam_target": ([_vp, _i, _i, _i, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_warp3d": ([_vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp], C.c_int),
+    "b200seg_warp3d_bwd": ([_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
@@ -192,7 +198,7 @@ def load_library(path: Optional[str] = None):
             fn = getattr(lib, name)          # AttributeError if the symbol is not exported
             fn.argtypes = argtypes
             fn.restype = restype
-        if lib.b200seg_version() < 200:
+        if lib.b200seg_version() < 201:
             raise RuntimeError("libb200seg.so is older than the Python binding")
         if path is None:
             _lib = lib
@@ -555,13 +561,14 @@ class CudaBackend:
         d1, d2, dr, do = _desc(y1), _desc(y2), _desc(res), _desc(out)
         self._check(self.lib.b200seg_apply(C.byref(d1), c1.data_ptr(), _ref(d2), _p(c2), _ref(dr), C.byref(do), dev, st))
 
-    # fused-coefficient forms: gn = (stats, gamma, beta, scale|None, vox, groups, eps)
+    # fused-coefficient forms: gn = (stats, gamma, beta, scale|None, vox, groups, eps[, act]); act defaults to ACT_RELU
     @staticmethod
     def _gn(gn):
         if gn is None:
             return None
-        stats, gamma, beta, scale, vox, groups, eps = gn
-        return GnDesc(stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), _p(scale), groups, vox, eps)
+        stats, gamma, beta, scale, vox, groups, eps = gn[:7]
+        act = gn[7] if len(gn) > 7 else ACT_RELU
+        return GnDesc(stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), _p(scale), groups, vox, eps, act)
 
     def apply_gn(self, y1, gn1, y2, gn2, res, out):
         dev, st = self._ds(y1)
@@ -901,6 +908,24 @@ class CudaBackend:
             sn, sc, sh, sw = img.stride()
             return (2, n, c, 1, h, w), (C.c_int64 * 5)(sn, sc, 0, sh, sw)
         return (3,) + tuple(img.shape), (C.c_int64 * 5)(*img.stride())
+
+    # ------------------------------------------------------------------ voxelmorph warp (csrc/warp3d.cu)
+    def warp3d(self, ddf, image, label, moved_image, moved_label):
+        """ddf fp32 contiguous (N, D, H, W, 3); image / label fp32 contiguous (N, C, D, H, W) or None; the moved
+        tensors likewise"""
+        dev, st = self._ds(ddf)
+        n, d, h, w = ddf.shape[:4]
+        ci = image.shape[1] if image is not None else 0
+        cl = label.shape[1] if label is not None else 0
+        self._check(self.lib.b200seg_warp3d(ddf.data_ptr(), _p(image), ci, _p(label), cl, n, d, h, w, _p(moved_image),
+                                            _p(moved_label), dev, st))
+
+    def warp3d_bwd(self, ddf, image, gmoved, addend, gddf):
+        """gddf (N, D, H, W, 3) = d loss / d ddf from gmoved (N, C, D, H, W) [+ addend (N, D, H, W, 3)]"""
+        dev, st = self._ds(ddf)
+        n, d, h, w = ddf.shape[:4]
+        self._check(self.lib.b200seg_warp3d_bwd(ddf.data_ptr(), image.data_ptr(), image.shape[1], gmoved.data_ptr(),
+                                                _p(addend), n, d, h, w, gddf.data_ptr(), dev, st))
 
     def ssim_fwd(self, img1, img2, window_size, taps, coef):
         """img1, img2 fp32 of one shape, any strides; taps fp32 host [window_size]; coef fp64 [4][map voxels] or None.

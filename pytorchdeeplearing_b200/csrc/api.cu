@@ -233,6 +233,9 @@ using namespace b200seg;
 #define ST(s) static_cast<cudaStream_t>(s)
 #define REQ_TENSOR(t, what) B200_CHECK_ARG(valid_tensor(t), "%s: invalid tensor descriptor '%s'", __func__, what)
 #define OPT_TENSOR(t, what) B200_CHECK_ARG((t) == nullptr || valid_tensor(t), "%s: invalid tensor descriptor '%s'", __func__, what)
+// the fused families (halo-convolution backward sums, stem_gn, up_gn) have the ReLU tail only
+#define REQ_RELU(gn) \
+  B200_CHECK_ARG((gn) == nullptr || (gn)->act == B200SEG_ACT_RELU, "%s: only B200SEG_ACT_RELU is supported", __func__)
 
 extern "C" {
 
@@ -378,6 +381,7 @@ int b200seg_conv_bwdstats(int kind, int dims, const b200seg_tensor* x, const voi
   OPT_TENSOR(addend, "addend");
   B200_CHECK_ARG(wpk != nullptr && gn != nullptr && sums != nullptr && gn->stats && gn->gamma && gn->beta,
                  "b200seg_conv_bwdstats: null argument");
+  REQ_RELU(gn);
   B200_CHECK_ARG(b200seg_conv_bwdstats_supported(kind, dims, x, w_dtype, y, addend, yfwd),
                  "b200seg_conv_bwdstats: unsupported shape (query b200seg_conv_bwdstats_supported first)");
   B200_DEVICE(device);
@@ -454,8 +458,11 @@ int b200seg_apply(const b200seg_tensor* y1, const float* coef1, const b200seg_te
   return ew_apply(y1, coef1, nullptr, y2, coef2, nullptr, res, out, device, ST(stream));
 }
 
+// The ReLU kernels derive one group per thread (GroupNorm(8) nets: at most 256 groups); the LeakyReLU kernels take
+// any number of groups up to 512 (InstanceNorm: one group per channel).
 static bool valid_gn(const b200seg_gn* g, int C) {
-  return g && g->stats && g->gamma && g->beta && g->groups > 0 && (C % g->groups) == 0 && g->vox > 0;
+  return g && g->stats && g->gamma && g->beta && g->groups > 0 && (C % g->groups) == 0 && g->vox > 0 &&
+         ((g->act == B200SEG_ACT_RELU && g->groups <= 256) || (g->act == B200SEG_ACT_LEAKY && g->groups <= 512));
 }
 
 int b200seg_apply_gn(const b200seg_tensor* y1, const b200seg_gn* gn1, const b200seg_tensor* y2, const b200seg_gn* gn2,
@@ -464,7 +471,8 @@ int b200seg_apply_gn(const b200seg_tensor* y1, const b200seg_gn* gn1, const b200
   REQ_TENSOR(out, "out");
   OPT_TENSOR(y2, "y2");
   OPT_TENSOR(res, "res");
-  B200_CHECK_ARG(valid_gn(gn1, y1->c) && (!y2 || valid_gn(gn2, y2->c)), "b200seg_apply_gn: bad GroupNorm reference");
+  B200_CHECK_ARG(valid_gn(gn1, y1->c) && (!y2 || (valid_gn(gn2, y2->c) && gn2->act == gn1->act)),
+                 "b200seg_apply_gn: bad GroupNorm reference");
   B200_DEVICE(device);
   return ew_apply(y1, nullptr, gn1, y2, nullptr, gn2, res, out, device, ST(stream));
 }
@@ -562,6 +570,8 @@ int b200seg_stem_gn_apply(const b200seg_tensor* x, const void* w3, const float* 
                           b200seg_stream stream) {
   REQ_TENSOR(x, "x");
   REQ_TENSOR(out, "out");
+  REQ_RELU(gn3);
+  REQ_RELU(gn1);
   B200_DEVICE(device);
   return stem_gn(1, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, out, nullptr, nullptr, nullptr, nullptr, nullptr,
                  nullptr, nullptr, nullptr, nullptr, device, ST(stream));
@@ -572,6 +582,8 @@ int b200seg_stem_gn_bwd_sums(const b200seg_tensor* x, const void* w3, const floa
                              double* sums1, int device, b200seg_stream stream) {
   REQ_TENSOR(x, "x");
   REQ_TENSOR(g, "g");
+  REQ_RELU(gn3);
+  REQ_RELU(gn1);
   B200_DEVICE(device);
   return stem_gn(2, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, nullptr, g, sums3, sums1, nullptr, nullptr, nullptr,
                  nullptr, nullptr, nullptr, device, ST(stream));
@@ -583,6 +595,8 @@ int b200seg_stem_gn_bwd(const b200seg_tensor* x, const void* w3, const float* b3
                         float* db1, int device, b200seg_stream stream) {
   REQ_TENSOR(x, "x");
   REQ_TENSOR(g, "g");
+  REQ_RELU(gn3);
+  REQ_RELU(gn1);
   B200_DEVICE(device);
   return stem_gn(3, x, w3, b3, w1, b1, gn3, gn1, nullptr, nullptr, nullptr, g, const_cast<double*>(sums3),
                  const_cast<double*>(sums1), dw3, dw1, dgamma, dbeta, db3, db1, device, ST(stream));
@@ -605,6 +619,7 @@ int b200seg_up_gn_apply(const b200seg_tensor* x, const void* w, const float* bia
                         const b200seg_tensor* out, int device, b200seg_stream stream) {
   REQ_TENSOR(x, "x");
   REQ_TENSOR(out, "out");
+  REQ_RELU(gn);
   B200_DEVICE(device);
   return up_gn(1, x, w, bias, gn, nullptr, out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, device,
                ST(stream));
@@ -614,6 +629,7 @@ int b200seg_up_gn_bwd_sums(const b200seg_tensor* x, const void* w, const float* 
                            const b200seg_tensor* g, double* sums, int device, b200seg_stream stream) {
   REQ_TENSOR(x, "x");
   REQ_TENSOR(g, "g");
+  REQ_RELU(gn);
   B200_DEVICE(device);
   return up_gn(2, x, w, bias, gn, nullptr, nullptr, g, sums, nullptr, nullptr, nullptr, nullptr, nullptr, device,
                ST(stream));
@@ -625,6 +641,7 @@ int b200seg_up_gn_bwd(const b200seg_tensor* x, const void* w, const float* bias,
   REQ_TENSOR(x, "x");
   REQ_TENSOR(g, "g");
   REQ_TENSOR(dx, "dx");
+  REQ_RELU(gn);
   B200_DEVICE(device);
   return up_gn(3, x, w, bias, gn, nullptr, nullptr, g, const_cast<double*>(sums), dw, dx, dgamma, dbeta, dbias, device,
                ST(stream));

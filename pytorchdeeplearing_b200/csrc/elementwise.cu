@@ -319,7 +319,7 @@ template <typename T> struct Vec<T, 1> {
   const long long vstep = stride / G; /* stride is a multiple of G */          \
   (void)total;
 
-template <typename T, int VEC>
+template <typename T, int VEC, int ACT>
 __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1, long long ld1,
                                                     const float* __restrict__ coef1, const T* __restrict__ y2,
                                                     long long ld2, const float* __restrict__ coef2,
@@ -335,9 +335,9 @@ __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1,
     double* s_d = s_dyn;                                                  // scratch doubles
     float* s_f = reinterpret_cast<float*>(s_d + gn_cta_doubles(C, gn1.groups > gn2.groups ? gn1.groups : gn2.groups, false));
     float* s_cf = s_f + 3 * C;                                            // [4][C]: A1, B1, A2, B2
-    gn_coefs<false, true>(GnCta(), gn1, nullptr, n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
+    gn_coefs<false, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn1, nullptr, n, C, s_d, s_f, s_cf, s_cf + C, nullptr, nullptr, nullptr);
     if (y2 != nullptr)
-      gn_coefs<false, true>(GnCta(), gn2, nullptr, n, C, s_d, s_f, s_cf + 2 * C, s_cf + 3 * C, nullptr, nullptr,
+      gn_coefs<false, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn2, nullptr, n, C, s_d, s_f, s_cf + 2 * C, s_cf + 3 * C, nullptr, nullptr,
                             nullptr);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
@@ -371,16 +371,16 @@ __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1,
     Vec<T, VEC>::load(y1 + v1 * ld1 + c0, a1);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      o0[j] = fmaxf(fmaf(a0[j], A1[j], B1[j]), 0.f);
-      o1[j] = fmaxf(fmaf(a1[j], A1[j], B1[j]), 0.f);
+      o0[j] = gn_act<ACT>(fmaf(a0[j], A1[j], B1[j]));
+      o1[j] = gn_act<ACT>(fmaf(a1[j], A1[j], B1[j]));
     }
     if (y2 != nullptr) {
       Vec<T, VEC>::load(y2 + v0 * ld2 + c0, a0);
       Vec<T, VEC>::load(y2 + v1 * ld2 + c0, a1);
 #pragma unroll
       for (int j = 0; j < VEC; ++j) {
-        o0[j] += fmaxf(fmaf(a0[j], A2[j], B2[j]), 0.f);
-        o1[j] += fmaxf(fmaf(a1[j], A2[j], B2[j]), 0.f);
+        o0[j] += gn_act<ACT>(fmaf(a0[j], A2[j], B2[j]));
+        o1[j] += gn_act<ACT>(fmaf(a1[j], A2[j], B2[j]));
       }
     }
     if (res != nullptr) {
@@ -400,11 +400,11 @@ __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1,
     float a[VEC], o[VEC];
     Vec<T, VEC>::load(y1 + vox * ld1 + c0, a);
 #pragma unroll
-    for (int j = 0; j < VEC; ++j) o[j] = fmaxf(fmaf(a[j], A1[j], B1[j]), 0.f);
+    for (int j = 0; j < VEC; ++j) o[j] = gn_act<ACT>(fmaf(a[j], A1[j], B1[j]));
     if (y2 != nullptr) {
       Vec<T, VEC>::load(y2 + vox * ld2 + c0, a);
 #pragma unroll
-      for (int j = 0; j < VEC; ++j) o[j] += fmaxf(fmaf(a[j], A2[j], B2[j]), 0.f);
+      for (int j = 0; j < VEC; ++j) o[j] += gn_act<ACT>(fmaf(a[j], A2[j], B2[j]));
     }
     if (res != nullptr) {
       Vec<T, VEC>::load(res + vox * ldr + c0, a);
@@ -421,7 +421,7 @@ __global__ void __launch_bounds__(256, 3) apply_kernel(const T* __restrict__ y1,
 // that -- across the 8 warps, across CTAs -- is accumulated in fp64 in a fixed order (one private shared-memory
 // row per warp, then ONE fp64 global atomic per (channel, sum) per CTA).  The grid is sized to the resident CTAs
 // (3 per SM) and the voxel loop keeps two trips of loads in flight: the kernel is a pure HBM stream.
-template <typename T, int VEC, bool DEEP>
+template <typename T, int VEC, bool DEEP, int ACT>
 __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const T* __restrict__ g, long long ldg,
                                                                const T* __restrict__ y, long long ldy,
                                                                const float* __restrict__ coef,
@@ -440,7 +440,7 @@ __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const 
   float A[VEC], B[VEC];
   float f1[VEC], f2[VEC], f3[VEC];
   if (gn.stats != nullptr) {
-    gn_coefs<false, true>(GnCta(), gn, nullptr, n, C, s_cd, s_cfl, s_ab, s_ab + C, nullptr, nullptr, nullptr);
+    gn_coefs<false, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn, nullptr, n, C, s_cd, s_cfl, s_ab, s_ab + C, nullptr, nullptr, nullptr);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
       A[j] = s_ab[c0 + j];
@@ -474,7 +474,7 @@ __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const 
       for (int u = 0; u < 4; ++u)
 #pragma unroll
         for (int j = 0; j < VEC; ++j) {
-          const float d = fmaf(ya[u][j], A[j], B[j]) > 0.f ? ga[u][j] : 0.f;
+          const float d = gn_act_bwd<ACT>(fmaf(ya[u][j], A[j], B[j]), ga[u][j]);
           f1[j] += d;
           f2[j] = fmaf(d, ya[u][j], f2[j]);
           f3[j] += ya[u][j];
@@ -489,8 +489,8 @@ __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const 
     Vec<T, VEC>::load(gb + (vi + vstep) * ldg, g1);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      const float d0 = fmaf(y0[j], A[j], B[j]) > 0.f ? g0[j] : 0.f;
-      const float d1 = fmaf(y1[j], A[j], B[j]) > 0.f ? g1[j] : 0.f;
+      const float d0 = gn_act_bwd<ACT>(fmaf(y0[j], A[j], B[j]), g0[j]);
+      const float d1 = gn_act_bwd<ACT>(fmaf(y1[j], A[j], B[j]), g1[j]);
       f1[j] += d0 + d1;
       f2[j] = fmaf(d0, y0[j], fmaf(d1, y1[j], f2[j]));
       f3[j] += y0[j] + y1[j];
@@ -502,7 +502,7 @@ __global__ void __launch_bounds__(256, DEEP ? 2 : 3) gn_bwd_reduce_kernel(const 
     Vec<T, VEC>::load(gb + vi * ldg, gv);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      const float d = fmaf(yv[j], A[j], B[j]) > 0.f ? gv[j] : 0.f;
+      const float d = gn_act_bwd<ACT>(fmaf(yv[j], A[j], B[j]), gv[j]);
       f1[j] += d;
       f2[j] = fmaf(d, yv[j], f2[j]);
       f3[j] += yv[j];
@@ -603,7 +603,7 @@ __global__ void gn_bwd_finalize_kernel(const double* __restrict__ sums, const fl
 }
 
 
-template <typename T, int VEC>
+template <typename T, int VEC, int ACT>
 __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restrict__ g, long long ldg,
                                                            const T* __restrict__ y, long long ldy,
                                                            const float* __restrict__ coef,
@@ -620,7 +620,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
     double* s_d = s_dyn;
     float* s_f = reinterpret_cast<float*>(s_d + gn_cta_doubles(C, gn.groups, true));
     float* s_c5 = s_f + 3 * C;                            // [5][C]: A, B, P, Q, R
-    const double* grp = gn_coefs<true, true>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
+    const double* grp = gn_coefs<true, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
                                              s_c5 + 3 * C, s_c5 + 4 * C);
     // parameter gradients (d gamma, d beta, d bias): ONE block per sample adds its sample's share from the
     // coefficients it has just derived (no serial loop over the batch at the tail of the grid); fp32 atomics over N
@@ -655,8 +655,8 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
     Vec<T, VEC>::load(g + v1 * ldg + c0, g1);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      const float d0 = fmaf(y0[j], A[j], B[j]) > 0.f ? g0[j] * P[j] : 0.f;
-      const float d1 = fmaf(y1[j], A[j], B[j]) > 0.f ? g1[j] * P[j] : 0.f;
+      const float d0 = gn_act_bwd_p<ACT>(fmaf(y0[j], A[j], B[j]), g0[j], P[j]);
+      const float d1 = gn_act_bwd_p<ACT>(fmaf(y1[j], A[j], B[j]), g1[j], P[j]);
       g0[j] = d0 + fmaf(y0[j], Q[j], R[j]);
       g1[j] = d1 + fmaf(y1[j], Q[j], R[j]);
     }
@@ -670,7 +670,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
     Vec<T, VEC>::load(g + vox * ldg + c0, gv);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      float d = fmaf(yv[j], A[j], B[j]) > 0.f ? gv[j] * P[j] : 0.f;
+      float d = gn_act_bwd_p<ACT>(fmaf(yv[j], A[j], B[j]), gv[j], P[j]);
       o[j] = d + fmaf(yv[j], Q[j], R[j]);
     }
     Vec<T, VEC>::store(dy + vox * ldd + c0, o);
@@ -682,7 +682,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_apply_kernel(const T* __restric
 // data; the tensors stay in L2 between the phases.  Requirements (checked by the host): every CTA of the grid is
 // resident at the same time (grid <= SMs x occupancy), channel groups are a power of two <= 256 (the staged
 // reduction), fused coefficients.  `counter` is a zero-initialised word owned by this launch (one-shot barrier).
-template <typename T, int VEC>
+template <typename T, int VEC, int ACT>
 __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restrict__ g, long long ldg,
                                                               const T* __restrict__ y, long long ldy,
                                                               T* __restrict__ dy, long long ldd, double* sums,
@@ -700,7 +700,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
   const T* gb = g + (long long)n * V * ldg + c0;
   float A[VEC], B[VEC];
   // ---------------------------------------------------------------- phase 1: per-(n, c) sums
-  gn_coefs<false, true>(GnCta(), gn, nullptr, n, C, s_d, s_f, s_c5, s_c5 + C, nullptr, nullptr, nullptr);
+  gn_coefs<false, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn, nullptr, n, C, s_d, s_f, s_c5, s_c5 + C, nullptr, nullptr, nullptr);
   float f1[VEC], f2[VEC], f3[VEC];
 #pragma unroll
   for (int j = 0; j < VEC; ++j) {
@@ -714,7 +714,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
     Vec<T, VEC>::load(gb + v * ldg, gv);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      const float d = fmaf(yv[j], A[j], B[j]) > 0.f ? gv[j] : 0.f;
+      const float d = gn_act_bwd<ACT>(fmaf(yv[j], A[j], B[j]), gv[j]);
       f1[j] += d;
       f2[j] = fmaf(d, yv[j], f2[j]);
       f3[j] += yv[j];
@@ -761,7 +761,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
   __syncthreads();
   // ---------------------------------------------------------------- phase 2: dy and the parameter gradients
   float P[VEC], Q[VEC], R[VEC];
-  const double* grp = gn_coefs<true, true>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
+  const double* grp = gn_coefs<true, true, GnCta, ACT != B200SEG_ACT_RELU>(GnCta(), gn, sums, n, C, s_d, s_f, s_c5, s_c5 + C, s_c5 + 2 * C,
                                            s_c5 + 3 * C, s_c5 + 4 * C);
   if (blockIdx.x == gridDim.x - 1) param_grads_of_sample(gn, sums, grp, s_f, n, C, dgamma, dbeta, dbias);
 #pragma unroll
@@ -779,7 +779,7 @@ __global__ void __launch_bounds__(256, 3) gn_bwd_fused_kernel(const T* __restric
     Vec<T, VEC>::load(gb + v * ldg, gv);
 #pragma unroll
     for (int j = 0; j < VEC; ++j) {
-      const float d = fmaf(yv[j], A[j], B[j]) > 0.f ? gv[j] * P[j] : 0.f;
+      const float d = gn_act_bwd_p<ACT>(fmaf(yv[j], A[j], B[j]), gv[j], P[j]);
       o[j] = d + fmaf(yv[j], Q[j], R[j]);
     }
     Vec<T, VEC>::store(db_ + v * ldd, o);
@@ -1020,9 +1020,13 @@ int ew_apply(const b200seg_tensor* y1, const float* c1, const b200seg_gn* g1, co
     const int mg = (g1 && g2 && g2->groups > g1->groups) ? g2->groups : (g1 ? g1->groups : 1);
     // (precomputed-coefficient form: no coefficient scratch -- any channel count fits)
     const size_t smem = (g1 && g1->stats) ? gn_cta_doubles(C, mg, false) * sizeof(double) + (size_t)7 * C * sizeof(float) : 0;
-    launch_k(apply_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(y1->ptr), y1->ld, c1, y2 ? static_cast<const T*>(y2->ptr) : nullptr, y2 ? y2->ld : 0, c2,
-        res ? static_cast<const T*>(res->ptr) : nullptr, res ? res->ld : 0, static_cast<T*>(out->ptr), out->ld, C, V,
-        gn_ref(g1, C), gn_ref(g2, C));
+    auto go = [&](auto kernel) {
+      launch_k(kernel, grid, 256, smem, s, static_cast<const T*>(y1->ptr), y1->ld, c1, y2 ? static_cast<const T*>(y2->ptr) : nullptr, y2 ? y2->ld : 0, c2,
+          res ? static_cast<const T*>(res->ptr) : nullptr, res ? res->ld : 0, static_cast<T*>(out->ptr), out->ld, C, V,
+          gn_ref(g1, C), gn_ref(g2, C));
+    };
+    if (g1 && g1->act == B200SEG_ACT_LEAKY) go(apply_kernel<T, VEC, B200SEG_ACT_LEAKY>);
+    else go(apply_kernel<T, VEC, B200SEG_ACT_RELU>);
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
@@ -1046,12 +1050,15 @@ int ew_gn_bwd_reduce(const b200seg_tensor* g, const b200seg_tensor* y, const flo
     const int staged = (pow2g && G <= 32 && staged_bytes <= 46 * 1024) ? 1 : 0;
     // precomputed-coefficient form without staging: only the [3][C] fp64 accumulators are touched (wide nets)
     const size_t base = (gn && gn->stats) ? full : (size_t)3 * C * sizeof(double);
+    auto go = [&](auto kernel) {
+      launch_k(kernel, grid, 256, staged ? staged_bytes : base, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, coef, sums, C, V,
+          gn_ref(gn, C), staged);
+    };
+    const bool leaky = gn && gn->act == B200SEG_ACT_LEAKY;
     if (deep)
-      launch_k(gn_bwd_reduce_kernel<T, VEC, true>, grid, 256, staged ? staged_bytes : base, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, coef, sums, C, V,
-          gn_ref(gn, C), staged);
+      leaky ? go(gn_bwd_reduce_kernel<T, VEC, true, B200SEG_ACT_LEAKY>) : go(gn_bwd_reduce_kernel<T, VEC, true, B200SEG_ACT_RELU>);
     else
-      launch_k(gn_bwd_reduce_kernel<T, VEC, false>, grid, 256, staged ? staged_bytes : base, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, coef, sums, C, V,
-          gn_ref(gn, C), staged);
+      leaky ? go(gn_bwd_reduce_kernel<T, VEC, false, B200SEG_ACT_LEAKY>) : go(gn_bwd_reduce_kernel<T, VEC, false, B200SEG_ACT_RELU>);
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
@@ -1084,10 +1091,12 @@ int ew_gn_bwd_apply(const b200seg_tensor* g, const b200seg_tensor* y, const floa
     const size_t smem = (gn && gn->stats) ? gn_cta_doubles(C, groups, true) * sizeof(double) + (size_t)8 * C * sizeof(float) : 0;
     GnRef gref = gn_ref(gn, C);
     gref.sum_y_from_stats = sum_y_from_stats;
-    launch_k(gn_bwd_apply_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld,
-                                                     static_cast<const T*>(y->ptr), y->ld, coef, coef3,
-                                                     static_cast<T*>(dy->ptr), dy->ld, C, V, gref, sums,
-                                                     y->n, dgamma, dbeta, dbias);
+    auto go = [&](auto kernel) {
+      launch_k(kernel, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld,
+               coef, coef3, static_cast<T*>(dy->ptr), dy->ld, C, V, gref, sums, y->n, dgamma, dbeta, dbias);
+    };
+    if (gn && gn->act == B200SEG_ACT_LEAKY) go(gn_bwd_apply_kernel<T, VEC, B200SEG_ACT_LEAKY>);
+    else go(gn_bwd_apply_kernel<T, VEC, B200SEG_ACT_RELU>);
   });
   B200_LAUNCH_CHECK();
   return B200SEG_OK;
@@ -1115,12 +1124,13 @@ int ew_gn_bwd_fused(const b200seg_tensor* g, const b200seg_tensor* y, const b200
   EW_DISPATCH(y, true, {
     const int G = C / VEC;
     const size_t smem = gn_cta_doubles(C, gn->groups, true) * sizeof(double) + (size_t)(8 + 24) * C * sizeof(float);
+    const bool leaky = gn->act == B200SEG_ACT_LEAKY;
+    auto kernel = leaky ? gn_bwd_fused_kernel<T, VEC, B200SEG_ACT_LEAKY> : gn_bwd_fused_kernel<T, VEC, B200SEG_ACT_RELU>;
     if (smem > 48 * 1024) {
-      static int attr_done[64] = {0};
-      if (device >= 0 && device < 64 && !attr_done[device]) {
-        B200_CUDA(cudaFuncSetAttribute(gn_bwd_fused_kernel<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       96 * 1024));
-        attr_done[device] = 1;
+      static int attr_done[2][64] = {{0}};
+      if (device >= 0 && device < 64 && !attr_done[leaky][device]) {
+        B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        attr_done[leaky][device] = 1;
       }
     }
     // all CTAs must be co-resident: cap the grid at one CTA per SM (the tensors are small)
@@ -1129,7 +1139,7 @@ int ew_gn_bwd_fused(const b200seg_tensor* g, const b200seg_tensor* y, const b200
     if ((256 % G) != 0) bx = (bx / G) * G;
     B200_CHECK_ARG(bx >= 1 && (long long)bx * y->n <= sms, "gn_bwd_fused: batch too large for a resident grid");
     dim3 grid(bx, y->n);
-    launch_k(gn_bwd_fused_kernel<T, VEC>, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, static_cast<T*>(dy->ptr), dy->ld,
+    launch_k(kernel, grid, 256, smem, s, static_cast<const T*>(g->ptr), g->ld, static_cast<const T*>(y->ptr), y->ld, static_cast<T*>(dy->ptr), dy->ld,
         sums, counter, C, V, gn_ref(gn, C), y->n, dgamma, dbeta, dbias);
   });
   B200_LAUNCH_CHECK();

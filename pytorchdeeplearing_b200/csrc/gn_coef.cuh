@@ -75,6 +75,27 @@ __host__ __device__ __forceinline__ double gn_dbias(double rstd, double ga, doub
   return rstd * ga * s1 + q * s3 + r * vox;
 }
 
+// The activation after the norm and dropout (B200SEG_ACT_*, a template parameter of the kernels that apply it), on the
+// pre-activation v = y*A + B: the forward value, and the backward factor on the incoming gradient g (torch's
+// threshold_backward / leaky_relu_backward, both keyed on the sign of v).  gn_act_bwd_p is g' * P with the ReLU form
+// written as the kernels always wrote it.  The LeakyReLU products are __fmul_rn: each is one rounding, never fused
+// into a neighbouring add.
+template <int ACT>
+__device__ __forceinline__ float gn_act(float v) {
+  if constexpr (ACT == B200SEG_ACT_LEAKY) return v > 0.f ? v : __fmul_rn(v, 0.01f);
+  else return fmaxf(v, 0.f);
+}
+template <int ACT>
+__device__ __forceinline__ float gn_act_bwd(float v, float g) {
+  if constexpr (ACT == B200SEG_ACT_LEAKY) return v > 0.f ? g : __fmul_rn(g, 0.01f);
+  else return v > 0.f ? g : 0.f;
+}
+template <int ACT>
+__device__ __forceinline__ float gn_act_bwd_p(float v, float g, float P) {
+  if constexpr (ACT == B200SEG_ACT_LEAKY) return __fmul_rn(v > 0.f ? g : __fmul_rn(g, 0.01f), P);
+  else return v > 0.f ? g * P : 0.f;
+}
+
 // The threads that derive the coefficients together, thread tid() of count(), and the barrier they meet at: the
 // whole CTA ...
 struct GnCta {
@@ -106,7 +127,7 @@ struct GnNamedBarrier {
 // registers.
 __host__ __device__ inline size_t gn_cta_doubles(int C, int groups, bool bwd) { return (size_t)(bwd ? 4 : 2) * C + 4 * groups; }
 
-template <bool BWD, bool STAGE, class Threads>
+template <bool BWD, bool STAGE, class Threads, bool WIDE = false>
 __device__ __forceinline__ double* gn_coefs(Threads th, const GnRef& r, const double* __restrict__ sums, int n, int C,
                                             double* s_d, float* s_f, float* A, float* B, float* P, float* Q,
                                             float* R) {
@@ -138,7 +159,23 @@ __device__ __forceinline__ double* gn_coefs(Threads th, const GnRef& r, const do
     }
   }
   th.sync();
-  if (th.tid() < r.groups) {
+  // one group per thread (the group loops are written twice so that the one-per-thread form, which every ReLU kernel
+  // uses, compiles exactly as it always has); WIDE: any number of groups (InstanceNorm has one per channel, more than
+  // a CTA has threads)
+  if constexpr (WIDE) {
+#pragma unroll 1
+    for (int g = th.tid(); g < r.groups; g += th.count()) {
+      double s = 0.0, q = 0.0;
+      for (int k = 0; k < cpg; ++k) {
+        s += d0[g * cpg + k];
+        q += d1[g * cpg + k];
+      }
+      double mean, rstd;
+      gn_mean_rstd(s, q, r.m, r.eps, mean, rstd);
+      grp[g * GS + 0] = mean;
+      grp[g * GS + 1] = rstd;
+    }
+  } else if (th.tid() < r.groups) {
     const int g = th.tid();
     double s = 0.0, q = 0.0;
     for (int k = 0; k < cpg; ++k) {
@@ -172,7 +209,18 @@ __device__ __forceinline__ double* gn_coefs(Threads th, const GnRef& r, const do
   }
   if (BWD) {
     th.sync();
-    if (th.tid() < r.groups) {
+    if constexpr (WIDE) {
+#pragma unroll 1
+      for (int g = th.tid(); g < r.groups; g += th.count()) {
+        double sa = 0.0, sax = 0.0;
+        for (int k = 0; k < cpg; ++k) {
+          sa += d2[g * cpg + k];
+          sax += d3[g * cpg + k];
+        }
+        grp[g * 4 + 2] = sa / r.m;
+        grp[g * 4 + 3] = sax / r.m;
+      }
+    } else if (th.tid() < r.groups) {
       const int g = th.tid();
       double sa = 0.0, sax = 0.0;
       for (int k = 0; k < cpg; ++k) {

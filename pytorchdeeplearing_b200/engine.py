@@ -33,6 +33,28 @@ K3, K1, DOWN, UP = 0, 1, 2, 3
 GROUPS = 8
 GN_EPS = 1e-5
 P_DROP = 0.2
+ACT_RELU, ACT_LEAKY = 0, 1     # activation after the norm (B200SEG_ACT_*)
+
+
+@dataclass(frozen=True)
+class VNetSpec:
+    """What distinguishes the VNet-shaped layer programs: LUConv ops per DownTransition / UpTransition (in pyramid
+    order, up_tr256 first), the parameter names of the norms and the LUConv convolutions, the norm's groups (0: one
+    per channel, InstanceNorm3d) and the activation."""
+    down_ops: Tuple[int, ...] = (2, 3, 3, 3)
+    up_ops: Tuple[int, ...] = (3, 3, 2, 1)
+    in_bn: str = "bn1"          # in_tr.<in_bn>
+    down_bn: str = "bn1"        # down_trX.<down_bn>
+    op_conv: str = "conv1"      # X.ops.j.<op_conv>
+    op_bn: str = "bn1"          # X.ops.j.<op_bn>
+    groups: int = GROUPS
+    act: int = ACT_RELU
+
+
+VNET = VNetSpec()
+# VNet3dRegistration (networks/VNet3dregistration.py:48-169): InstanceNorm3d(affine) and LeakyReLU(0.01)
+REGISTRATION = VNetSpec(down_ops=(2, 2, 2, 2), up_ops=(2, 2, 2, 1), in_bn="bn", down_bn="bn", op_conv="conv",
+                        op_bn="bn", groups=0, act=ACT_LEAKY)
 # the ResNet stages whose outputs Grad-CAM can take (resnet_backward ``stages``), in forward order
 RESNET_STAGES = ("in_tr", "down_tr32", "down_tr64", "down_tr128", "down_tr256")
 
@@ -161,6 +183,7 @@ class Engine:
         self._deferred = None                  # (side, fork event, pack plan, zero buffers) not launched yet
         self._ov = 0                           # scheduling options of this pass (overlap_mask), fixed at forward
         self._data_only = False                # backward computes data gradients only (no weight-gradient convolutions)
+        self.spec = VNET                       # norm groups and activation of conv_gn (vnet_forward sets its spec)
 
     # ---------------------------------------------------------------- allocation helpers
     def new(self, like: Tensor, sp: Sequence[int], c: int, dtype=None) -> Tensor:
@@ -352,8 +375,13 @@ class Engine:
         if cout <= 512:
             # kernels derive the coefficients from the statistics themselves: no finalize launch
             # (wider layers -- init_features >= 64 -- take the finalize/apply form: any channel count)
-            L.gn = (stats, self.P[gname + ".weight"], self.P[gname + ".bias"], L.scale, vox, GROUPS, GN_EPS)
+            L.gn = (stats, self.P[gname + ".weight"], self.P[gname + ".bias"], L.scale, vox,
+                    self.spec.groups or cout, GN_EPS)
+            if self.spec.act != ACT_RELU:
+                L.gn += (self.spec.act,)
         else:
+            if self.spec != VNET:
+                raise ValueError(f"the InstanceNorm / LeakyReLU layers take at most 512 channels, got {cout}")
             L.coef = torch.empty((n, cout, 2), dtype=torch.float32, device=x.device)
             L.mr = torch.empty((n, GROUPS, 2), dtype=torch.float32, device=x.device)
             self.be.gn_finalize(stats, self.P[gname + ".weight"], self.P[gname + ".bias"], L.scale, vox,
@@ -365,7 +393,8 @@ class Engine:
         """can the input block run fused (``stem_block``)?  bf16 storage, one image channel, 16 features, and a backend
         with the fused kernels (the emulated CPU backend and the fp32 parity mode keep the per-branch calls)"""
         ok = getattr(self.be, "stem_gn_ok", None)
-        return ok is not None and self.T == torch.bfloat16 and f == 16 and ok(x, f, self.dims)
+        return (ok is not None and self.spec.act == ACT_RELU and self.spec.groups == GROUPS and self.T == torch.bfloat16
+                and f == 16 and ok(x, f, self.dims))
 
     def stem_block(self, x: Tensor, sp0, f: int, out: Tensor, drop: bool) -> Tuple[Layer, Layer]:
         """InputTransition (VNet3d.py:34-43, ResNet3d.py:24-41): relu(bn1(conv1(x))) + relu(bn1(conv2(x))) with the
@@ -416,7 +445,8 @@ class Engine:
         the pointwise mma.sync kernel, and a backend with the fused kernels (the emulated CPU backend and the fp32
         parity mode keep the per-layer calls)"""
         ok = getattr(self.be, "up_gn_ok", None)
-        if ok is None or self.T != torch.bfloat16 or self.dims != 3:
+        if ok is None or self.T != torch.bfloat16 or self.dims != 3 or self.spec.act != ACT_RELU \
+                or self.spec.groups != GROUPS:
             return False
         return ok(x, self._packs.get((wname, "fwd")), co, self.dims)
 
@@ -559,8 +589,10 @@ class Engine:
         if dx_out is None:
             dx_out = torch.empty(L.x.shape, dtype=self.T, device=dev)
         ok = getattr(be, "conv_bwdstats_ok", None)
+        # (the fused backward-sums epilogue has the ReLU tail only: a LeakyReLU layer takes the two-pass form)
         if (prev is not None and prev.gn is not None and prev.gname is not None and ok is not None
-                and prev.y.shape == dx_out.shape and ok(dkind, self.dims, dy, wd, dx_out, dx_addend, prev.y)):
+                and len(prev.gn) == 7 and prev.y.shape == dx_out.shape
+                and ok(dkind, self.dims, dy, wd, dx_out, dx_addend, prev.y)):
             self._tag(prev.wname)
             prev.pre_sums = self.zeros((prev.y.shape[0], prev.y.shape[-1], 3), torch.float64, dev)
             be.conv_bwdstats(dkind, self.dims, dy, wd, dx_out, dx_addend, prev.y, prev.gn, prev.pre_sums)
@@ -620,11 +652,16 @@ class Engine:
         return logits[:, 0].permute(0, 3, 1, 2), (probs[:, 0].permute(0, 3, 1, 2) if probs is not None else None)
 
     def vnet_forward(self, P: Dict[str, Tensor], x: Tensor, masks: Optional[List[Tensor]],
-                     need_grad: bool) -> Tuple[Tensor, Tensor]:
+                     need_grad: bool, spec: VNetSpec = VNET) -> Tuple[Tensor, Tensor]:
         """VNet3d.forward (reference networks/VNet3d.py:129-158) and its 2-D twin VNet2d.forward
         (networks/VNet2d.py:129-158; 2-D tensors run with a unit depth).  ``x``: (N,Cin,[D,]H,W) fp32.
-        Returns channels-last-strided (N,ncls,[D,]H,W) fp32 logits and probs."""
+        Returns channels-last-strided (N,ncls,[D,]H,W) fp32 logits and probs.  ``spec=REGISTRATION``: the network of
+        VNet3dRegistration up to its displacement field (networks/VNet3dregistration.py:174-203)."""
         self.P, self.masks, self._mi, self.layers, self.need_grad = P, masks, 0, [], need_grad
+        self.spec = spec
+        oc, ob = spec.op_conv, spec.op_bn
+        downs = tuple(zip(("down_tr32", "down_tr64", "down_tr128", "down_tr256"), spec.down_ops))
+        ups = tuple(zip(("up_tr256", "up_tr128", "up_tr64", "up_tr32"), spec.up_ops))
         sv = self.saved = {}
         dims = self.dims
         n, cin = x.shape[0], x.shape[1]
@@ -649,13 +686,13 @@ class Engine:
 
         vox = [sp[0] * sp[1] * sp[2] for sp in sps]
         specs = [("in_tr.conv1.weight", K3, vox[0], vox[0], False), ("in_tr.conv2.weight", K1, vox[0], vox[0], False)]
-        for i, (name, nops) in enumerate((("down_tr32", 2), ("down_tr64", 3), ("down_tr128", 3), ("down_tr256", 3))):
+        for i, (name, nops) in enumerate(downs):
             specs.append((name + ".down_conv.weight", DOWN, vox[i + 1], vox[i], True))
-            specs += [(f"{name}.ops.{j}.conv1.weight", K3, vox[i + 1], vox[i + 1], True) for j in range(nops)]
-        for i, (name, nops) in zip((3, 2, 1, 0), (("up_tr256", 3), ("up_tr128", 3), ("up_tr64", 2), ("up_tr32", 1))):
+            specs += [(f"{name}.ops.{j}.{oc}.weight", K3, vox[i + 1], vox[i + 1], True) for j in range(nops)]
+        for i, (name, nops) in zip((3, 2, 1, 0), ups):
             specs.append((name + ".up_conv.weight", UP, vox[i], vox[i + 1], True))
             specs.append((name + ".conv.weight", K1, vox[i], vox[i], True))
-            specs += [(f"{name}.ops.{j}.conv1.weight", K3, vox[i], vox[i], True) for j in range(nops)]
+            specs += [(f"{name}.ops.{j}.{oc}.weight", K3, vox[i], vox[i], True) for j in range(nops)]
         self._batch, self._ov = n, overlap_mask("vnet", dims)
         self._prepack(specs, need_grad, n_early=5)         # in_tr (2) + down_tr32 (down conv + 2 ops)
 
@@ -664,23 +701,24 @@ class Engine:
             La, Lb = self.stem_block(xin, sp0, f, skips[0], drop=True)
             out = skips[0]
         else:
-            La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", "in_tr.bn1", xin, sp0, f)
-            Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", "in_tr.bn1", xin, sp0, f)
+            ib = "in_tr." + spec.in_bn
+            La = self.conv_gn(K3, "in_tr.conv1.weight", "in_tr.conv1.bias", ib, xin, sp0, f)
+            Lb = self.conv_gn(K1, "in_tr.conv2.weight", "in_tr.conv2.bias", ib, xin, sp0, f)
             out = self.act(La, skips[0], L2=Lb)
         sv["in_tr"] = (La, Lb)
 
         # ---- DownTransition3d x4 (VNet3d.py:55-59)
-        nconvs = {"down_tr32": 2, "down_tr64": 3, "down_tr128": 3, "down_tr256": 3}
-        for i, name in enumerate(["down_tr32", "down_tr64", "down_tr128", "down_tr256"]):
+        for i, (name, nops) in enumerate(downs):
             co, sp = ch[i + 1], sps[i + 1]
-            Ld = self.conv_gn(DOWN, name + ".down_conv.weight", name + ".down_conv.bias", name + ".bn1", out, sp, co)
+            Ld = self.conv_gn(DOWN, name + ".down_conv.weight", name + ".down_conv.bias", f"{name}.{spec.down_bn}",
+                              out, sp, co)
             down = self.act(Ld, self.new(x, sp, co))
             h, ops = down, []
-            for j in range(nconvs[name]):
-                Lo = self.conv_gn(K3, f"{name}.ops.{j}.conv1.weight", f"{name}.ops.{j}.conv1.bias",
-                                  f"{name}.ops.{j}.bn1", h, sp, co)
+            for j in range(nops):
+                Lo = self.conv_gn(K3, f"{name}.ops.{j}.{oc}.weight", f"{name}.ops.{j}.{oc}.bias",
+                                  f"{name}.ops.{j}.{ob}", h, sp, co)
                 ops.append(Lo)
-                last = j == nconvs[name] - 1
+                last = j == nops - 1
                 if last:
                     dst = skips[i + 1] if i + 1 < 4 else self.new(x, sp, co)
                     h = self.act(Lo, dst, res=down)                     # torch.add(out, down), VNet3d.py:58
@@ -690,8 +728,7 @@ class Engine:
             out = h
 
         # ---- UpTransition3d x4 (VNet3d.py:72-80)
-        nconvs = {"up_tr256": 3, "up_tr128": 3, "up_tr64": 2, "up_tr32": 1}
-        for i, name in zip((3, 2, 1, 0), ["up_tr256", "up_tr128", "up_tr64", "up_tr32"]):
+        for i, (name, nops) in zip((3, 2, 1, 0), ups):
             co, sp = ch[i], sps[i]
             if name == "up_tr32" and self.up_gn_ok(out, name + ".up_conv.weight", co):
                 Lu = self.up_block(name, out, sp, co, cats[i][..., :co])
@@ -701,11 +738,11 @@ class Engine:
             Lc = self.conv_gn(K1, name + ".conv.weight", name + ".conv.bias", name + ".bn", cats[i], sp, co)
             xcat = self.act(Lc, self.new(x, sp, co))
             h, ops = xcat, []
-            for j in range(nconvs[name]):
-                Lo = self.conv_gn(K3, f"{name}.ops.{j}.conv1.weight", f"{name}.ops.{j}.conv1.bias",
-                                  f"{name}.ops.{j}.bn1", h, sp, co)
+            for j in range(nops):
+                Lo = self.conv_gn(K3, f"{name}.ops.{j}.{oc}.weight", f"{name}.ops.{j}.{oc}.bias",
+                                  f"{name}.ops.{j}.{ob}", h, sp, co)
                 ops.append(Lo)
-                last = j == nconvs[name] - 1
+                last = j == nops - 1
                 h = self.act(Lo, self.new(x, sp, co), res=xcat if last else None)   # VNet3d.py:79
             sv[name] = (Lu, Lc, ops)
             out = h

@@ -48,6 +48,10 @@ class GraphedStep:
     def __init__(self, model: torch.nn.Module, lossfn, x: torch.Tensor, y: torch.Tensor, warmup: int = 2,
                  optimizer: Optional[torch.optim.Optimizer] = None, use_graph: bool = True,
                  want_probs: bool = False):
+        from .networks.VNet3dregistration import VNet3dRegistration
+        if isinstance(model, VNet3dRegistration):
+            raise TypeError("GraphedStep captures segmentation nets with a segmentation loss; VNet3dRegistration's "
+                            "loss is the caller's: train it eagerly")
         self.model, self.lossfn, self.optimizer = model, lossfn, optimizer
         self.want_probs = want_probs
         self.x = torch.empty_like(x)

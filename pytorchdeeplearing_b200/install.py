@@ -2,7 +2,8 @@
 
 The reference wrappers bind the classes at import time (``from networks.VNet3d import VNet3d``
 model/modelVNet.py:2-4, model/modelUnet.py:2-4; losses model/modelVNet.py:7-8), so ``install``
-rebinds those names in whichever of ``networks``, ``networks.*`` (``networks.Unet3dthin`` included), ``model.modelVNet``,
+rebinds those names in whichever of ``networks``, ``networks.*`` (``networks.Unet3dthin`` and
+``networks.VNet3dregistration`` included), ``model.modelVNet``,
 ``model.modelUnet``, ``model.modelResNet``, ``model.losses``, ``model.metric``, ``model.lossesSSIM``, ``model.lossescldice`` are already imported (and in ``sys.modules`` entries
 imported later via the same names).  The mask post-processing functions are rebound in ``dataprocess.utils``, and
 ``GradCAM`` in ``model.visualization`` and ``model.modelResNet`` (so ``Grad_CAM_Visual`` runs on the GPU).
@@ -18,7 +19,7 @@ import sys
 
 _SAVED = []
 
-_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet2d", "ResNet3d")
+_NET_NAMES = ("VNet3d", "VNet2d", "UNet3d", "UNet3dthin", "UNet2d", "ResNet2d", "ResNet3d", "VNet3dRegistration")
 _METRIC_NAMES = ("dice_coeff", "iou_coeff", "multiclass_dice_coeff", "multiclass_iou_coeff", "Seg_Metirc3d")
 _LOSS_NAMES = ("BinaryDiceLoss", "BinaryCrossEntropyLoss", "BinaryFocalLoss", "BinaryCrossEntropyDiceLoss",
                "MutilCrossEntropyLoss", "MutilFocalLoss", "MutilDiceLoss", "MutilCrossEntropyDiceLoss")
@@ -36,7 +37,7 @@ _MODULES = ("networks", "networks.VNet3d", "networks.VNet2d", "networks.Unet3d",
             "model.losses", "model.metric", "model.modelVNet", "model.modelUnet", "model.lossesSSIM",
             "model.lossescldice", "networks.ResNet2d", "networks.ResNet3d", "model.modelResNet",
             "dataprocess.Augmentation.images_masks_3dtransform", "dataprocess.Augmentation.ImageAugmentation",
-            "dataprocess.utils", "model.visualization", "dataprocess.AugData")
+            "dataprocess.utils", "model.visualization", "dataprocess.AugData", "networks.VNet3dregistration")
 
 
 def install() -> int:

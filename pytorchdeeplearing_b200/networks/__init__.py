@@ -8,6 +8,7 @@ from .VNet3d import VNet3d
 from .VNet2d import VNet2d
 from .ResNet2d import ResNet2d
 from .ResNet3d import ResNet3d
+from .VNet3dregistration import VNet3dRegistration
 
 
 def initialize_weights(net):
@@ -28,4 +29,4 @@ def initialize_weights(net):
         nn.init.constant_(net.bias.data, 0)
 
 
-__all__ = ["UNet2d", "UNet3d", "UNet3dthin", "VNet3d", "VNet2d", "ResNet2d", "ResNet3d", "initialize_weights"]
+__all__ = ["UNet2d", "UNet3d", "UNet3dthin", "VNet3d", "VNet2d", "ResNet2d", "ResNet3d", "VNet3dRegistration", "initialize_weights"]
