@@ -31,6 +31,7 @@ struct Cell {
   float w[8];
   int x0, y0, z0;
   float ix, iy, iz;
+  bool any;       // every coordinate passes coord_in_range: the weights are finite and some corners may be inside
 };
 
 // |coordinate| far beyond the volume: every corner is outside (and floor() stays within int range)
@@ -39,6 +40,7 @@ __device__ __forceinline__ bool coord_in_range(float u, int s) { return u > -2.f
 __device__ __forceinline__ void make_cell(float ix, float iy, float iz, int D, int H, int W, Cell& c) {
   c.ix = ix; c.iy = iy; c.iz = iz;
   const bool any = coord_in_range(ix, W) && coord_in_range(iy, H) && coord_in_range(iz, D);
+  c.any = any;
   const int x0 = any ? (int)floorf(ix) : -4, y0 = any ? (int)floorf(iy) : -4, z0 = any ? (int)floorf(iz) : -4;
   c.x0 = x0; c.y0 = y0; c.z0 = z0;
   const float fx0 = (float)x0, fy0 = (float)y0, fz0 = (float)z0;
@@ -120,9 +122,13 @@ __global__ void __launch_bounds__(256) warp3d_bwd_kernel(const float* __restrict
   const float ex = __fsub_rn((float)(c.x0 + 1), ix), wx = __fsub_rn(ix, fx0);
   const float ey = __fsub_rn((float)(c.y0 + 1), iy), wy = __fsub_rn(iy, fy0);
   const float ez = __fsub_rn((float)(c.z0 + 1), iz), wz = __fsub_rn(iz, fz0);
-  // d weight / d x, y, z of each corner (sign folded in below), grid_sample's gix / giy / giz accumulation
+  // d weight / d x, y, z of each corner (sign folded in below), grid_sample's gix / giy / giz accumulation.  A corner
+  // outside the volume adds val = 0 times finite factors, i.e. nothing, as torch skips it -- but only while every
+  // coordinate is in range: beyond it (|ddf| = inf, NaN) the factors are not finite and 0 * inf would be NaN, and
+  // every corner is outside, so the sample adds nothing at all.
   float gix = 0.f, giy = 0.f, giz = 0.f;
-  for (int ch = 0; ch < ci; ++ch) {
+  const int nch = c.any ? ci : 0;
+  for (int ch = 0; ch < nch; ++ch) {
     const float* src = image + ((long long)n * ci + ch) * V;
     const float go = gmoved[((long long)n * ci + ch) * V + v];
     float val[8];

@@ -8,6 +8,10 @@ Sampling positions are torch's own fp32 numbers (the reference's normalisation, 
 unnormalisation, without FMA contraction), so the nearest-sampled label is bit-identical to torch's and the trilinear
 image uses the same cells and weights.  As in torch, the nearest path passes no gradient to ``ddf``.
 
+A displacement of +-inf or NaN puts its sample outside the volume, as does any coordinate at or beyond -2 or s + 1:
+there the moved image and label are 0 and d loss / d ddf is exactly 0 (plus the addend), which is what torch's
+grid_sample and its autograd give on the GPU for the same coordinates.
+
 Differences from the reference, by design:
   * inputs must be fp32 CUDA tensors (``TypeError`` otherwise);
   * the moving image and label are data: neither may require a gradient (``ValueError``); the reference would

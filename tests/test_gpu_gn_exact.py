@@ -35,6 +35,7 @@ import torch
 import torch.nn.functional as F
 
 from emu_backend import K3
+from pytorchdeeplearing_b200._abi import ACT_LEAKY, ACT_RELU
 from test_gpu_conv_exact import Guarded, assert_guards, first_mismatch, assert_bitwise
 from test_gpu_conv_exact import C as conv_case, GUARD, IN_FILL, OUT_BITS, conv_geometry
 
@@ -117,18 +118,23 @@ def fused_supported(cs, sms=SMS):
             cs["n"] * math.prod(cs["sp"]) * cs["c"] <= 4 << 20 and cs["n"] <= sms)
 
 
-def reduce_staged(cs, gn_form):
+def reduce_staged(cs, gn_form, groups=GROUPS):
     """staged (elementwise.cu:1126-1130): power-of-two vector groups <= 32 and the staging rows fit in 46 KB"""
     C = cs["c"]
     G = C // (vec_width(cs["dtype"]) if vec_ok(cs) else 1)
-    groups = GROUPS if gn_form else 1
+    groups = groups if gn_form else 1
     full = (3 * C + 2 * C + 4 * groups) * 8 + 5 * C * 4
     return G & (G - 1) == 0 and G <= 32 and full + 8 * 3 * C * 4 <= 46 * 1024
 
 
-def ew_variants(cs):
-    """the kernel variants the case reaches (labels "kernel:variant")"""
+def ew_variants(cs, groups=GROUPS, act=ACT_RELU):
+    """the kernel variants the case reaches (labels "kernel:variant") with `groups` GroupNorm groups and activation
+    `act`.  The LeakyReLU tail exists only in the fused-coefficient forms (apply_gn, gn_bwd_apply_gn,
+    gn_bwd_reduce_gn, gn_bwd_fused_gn; C <= 512): the precomputed-coefficient forms and colsum reach nothing with it"""
     N, V, C = cs["n"], math.prod(cs["sp"]), cs["c"]
+    leaky = act == ACT_LEAKY
+    if leaky and C > 512:
+        return set()
     vec = vec_width(cs["dtype"]) if vec_ok(cs) else 1
     G = C // vec
     out = set()
@@ -146,15 +152,19 @@ def ew_variants(cs):
     t = tags + ["deep" if deep else "shallow"] + (["tail"] if any(k % 2 for k in cnt) else [])
     if deep and any(k % 4 >= 2 for k in cnt):
         t.append("deep_rem2")
-    t.append("staged" if reduce_staged(cs, False) else "atomic")
+    if not leaky:
+        t.append("staged" if reduce_staged(cs, False) else "atomic")
     if C <= 512:
-        t.append("gn_staged" if reduce_staged(cs, True) else "gn_atomic")
+        t.append("gn_staged" if reduce_staged(cs, True, groups) else "gn_atomic")
     out |= {f"reduce:{x}" for x in t}
     if fused_supported(cs):
         out.add("fused:" + ("narrow" if G <= 32 else "wide"))
-    out |= {f"colsum:{x}" for x in tags}
+    if not leaky:
+        out |= {f"colsum:{x}" for x in tags}
     if C > 512:
         out.add("coef:wide")
+    if groups > 256:
+        out.add("coef:groups>256")      # gn_coefs' WIDE group loops take a second trip over the 256 threads
     return out
 
 
@@ -165,6 +175,17 @@ REQUIRED_VARIANTS = {
     "reduce:staged", "reduce:atomic", "reduce:gn_staged", "reduce:gn_atomic", "reduce:round_g",
     "fused:narrow", "fused:wide", "colsum:vec8", "colsum:vec4", "colsum:vec1", "colsum:round_g", "coef:wide",
 }
+
+
+def required_variants(act):
+    """the labels the cases of activation `act` must reach.  LeakyReLU (InstanceNorm, groups = C; the cases of
+    test_gpu_gn_act_warp.py): every label of the fused-coefficient forms that the ReLU form requires, and more than
+    256 groups (the ReLU form refuses those)"""
+    if act == ACT_RELU:
+        return REQUIRED_VARIANTS
+    return {v for v in REQUIRED_VARIANTS
+            if v.split(":")[0] in ("apply", "bwd_apply", "reduce", "fused")
+            and v not in ("reduce:staged", "reduce:atomic")} | {"coef:groups>256"}
 
 
 # ---------------------------------------------------------------------------------------------------------- design
@@ -380,7 +401,7 @@ def decode_mask(s1, nbits, shift):
 # ---------------------------------------------------------------------------------------------------------- CPU part
 def test_every_kernel_variant_has_a_case():
     reached = set().union(*(ew_variants(c) for c in EW_CASES.values()))
-    assert REQUIRED_VARIANTS <= reached, sorted(REQUIRED_VARIANTS - reached)
+    assert required_variants(ACT_RELU) <= reached, sorted(required_variants(ACT_RELU) - reached)
 
 
 @pytest.mark.parametrize("name", sorted(EW_CASES))
